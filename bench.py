@@ -1,15 +1,18 @@
 #!/usr/bin/env python
 """bench.py -- training_step throughput of the HashGrid + FullyFusedMLP hot path (BASELINE.json configs[1]).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
 
 One "step" = one trainer->training_step (fused fwd+loss+bwd kernel + Adam) over one batch of 2^18 synthetic
 uniform-[0,1)^3 positions with closed-form targets. Prints ONE JSON line (rank 0). See DESIGN.md "Measurement".
 Own arm: N ranks (one per GPU, torchrun), batch sharded over ranks (global batch = N * 2^18 -> weak scaling), gradients
 all-reduced over NCCL before the (replicated) Adam step.
-Reference arm (--impl reference): the UNMODIFIED reference compiled into oracle/_ref/ref_harness (its sm_100 build, run
+Reference arm (--impl reference): the UNMODIFIED reference compiled into oracle/_ref/ref_harness (its sm_90 build, run
 on the GPU through its own C++ API; all three modes are timed and the fastest FullyFusedMLP mode is the line's value),
 plus the CPU oracle port on the host cores as cpu_baseline. The reference has no CPU implementation of this path.
+--dump-outputs DIR (own arm, rank 0): after the timed steps, what the last timed training step produced -- its loss, a fixed
+sample of the updated fp32 parameters and of the parameter gradients -- as DIR/<name>.npy, so that two builds can be compared
+output for output (the inputs are the same seeded batches in every run).
 """
 import argparse
 import json
@@ -33,7 +36,7 @@ FUSED_BYTES_PER_SAMPLE = 1048
 ADAM_BYTES_PER_PARAM = 36
 
 
-L2_NOTE = "per-step working set (tables+optimizer state ~770 MB) exceeds the 126 MB L2; 4 rotating input batches; no explicit flush"
+L2_NOTE = "per-step working set (tables+optimizer state ~770 MB) exceeds the 50 MB L2; 4 rotating input batches; no explicit flush"
 E2E_WARMUP = 10
 
 
@@ -47,11 +50,11 @@ def measured_peaks():
     if os.path.exists(path):
         d = json.load(open(path))
         return float(d["hbm_gbs"]), "measured"
-    return 6650.0, "fallback"
+    return 3350.0, "datasheet"  # H100 SXM HBM3
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md). NVML is initialised when the sampler is
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region. NVML is initialised when the sampler is
     created -- before the timed region -- so that even a region of a few milliseconds gets samples (one is taken synchronously on
     entry and one on exit, the thread adds one per millisecond in between)."""
 
@@ -164,7 +167,6 @@ def run_reference(args):
             "config": config_dict(1, "dp1")}  # the reference is a single-GPU library: one GPU whatever --gpus says
     modes = {}
     if os.path.exists(harness):
-        os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
         env = dict(os.environ)
         for name, cfg, jit in (("fully_fused", "headline.json", 0), ("fully_fused_jit", "headline.json", 1), ("cutlass", "headline_cutlass.json", 0)):
             cmd = [harness, "bench", os.path.join(ROOT, "tests", "golden", "configs", cfg), str(N_IN), str(N_OUT), str(BATCH), str(args.steps), str(args.warmup), str(jit)]
@@ -187,7 +189,7 @@ def run_reference(args):
                     final_loss=ok[best].get("loss_after_steps"))
         line["reference_modes"] = modes
         line["cpu_baseline"] = {"value": ok[best]["samples_per_s"], "unit": "samples/s", "cores": 0, "kind": "reference",
-                                "sample": f"the reference's own sm_100 build on the GPU ({best}); it has no CPU path. CPU oracle port: {cb['value']:.3e} samples/s on {cb['cores']} threads"}
+                                "sample": f"the reference's own sm_90 build on the GPU ({best}); it has no CPU path. CPU oracle port: {cb['value']:.3e} samples/s on {cb['cores']} threads"}
         line["cpu_oracle_port"] = cb
     else:
         # reference binary absent: the oracle port on the host cores is the only reference arm available
@@ -218,19 +220,6 @@ def run_reference(args):
             line["inference"] = {"error": repr(e)}
     line["gpu_launches"] = 0
     print(json.dumps(line))
-
-
-def ncu_traffic():
-    """DRAM bytes per launch of the dominant kernel from the committed ncu capture (profiles/r0N_traffic.json, newest round)."""
-    try:
-        for name in ("r02_traffic.json", "r01_traffic.json"):
-            path = os.path.join(ROOT, "profiles", name)
-            if os.path.exists(path):
-                t = json.load(open(path))
-                return {"kernel": t["kernel"], "bytes": t["dram_bytes_read_per_launch"] + t["dram_bytes_write_per_launch"], "source": "profiles/" + name}
-    except Exception:  # noqa: BLE001
-        pass
-    return {}
 
 
 def closed_form_targets(torch, x, n_out):
@@ -307,6 +296,8 @@ def run_own(args):
     prof = model.read_profile()
     model.set_profiling(False)
     launches = tcnn_b200.kernel_launch_count() - launches0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, model, dp.loss())
     # loss of training step number warmup + steps (one more step on the next batch of the pool): the reference arm prints the same
     # quantity after the same number of steps on the same data sequence (rank 0 draws the reference's pcg32{1337} stream)
     step(args.warmup + args.steps)
@@ -386,7 +377,6 @@ def run_own(args):
         binning_ms = prof["binning_ms_total"] / n_prof
         achieved = FUSED_BYTES_PER_SAMPLE * BATCH / (fused_ms * 1e-3) / 1e9 if fused_ms > 0 else 0.0
         ms_per_step = ms / args.steps
-        traffic = ncu_traffic()
         line = {
             "metric": METRIC, "value": global_batch * args.steps / (ms * 1e-3), "unit": "samples/s", "n_gpus": world, "steps": args.steps,
             "warmup": args.warmup, "ms_per_step": ms_per_step, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
@@ -400,9 +390,9 @@ def run_own(args):
             "strong_scaling": strong,
             "dp_engine": getattr(dp, "engine", "single"),
             "gpu_launches": int(launches),
-            "roofline": {"bound": "hbm", "kernel": traffic.get("kernel", "fused_ws_kernel"), "achieved": achieved, "peak": peak, "peak_kind": peak_kind, "unit": "GB/s",
-                         "frac": achieved / peak, "traffic": traffic.get("bytes"), "traffic_unit": "B/launch (ncu dram__bytes_read.sum + dram__bytes_write.sum)", "kernel_ms": fused_ms, "optimizer_kernel_ms": adam_ms, "binning_kernels_ms": binning_ms,
-                         # algorithmic 36 B/parameter (SURVEY.md section 8d); the zero-gradient skip moves fewer bytes (ncu: profiles/). Only
+            "roofline": {"bound": "hbm", "kernel": "fused_ws_kernel", "achieved": achieved, "peak": peak, "peak_kind": peak_kind, "unit": "GB/s",
+                         "frac": achieved / peak, "kernel_ms": fused_ms, "optimizer_kernel_ms": adam_ms, "binning_kernels_ms": binning_ms,
+                         # algorithmic 36 B/parameter (SURVEY.md section 8d); the zero-gradient skip moves fewer bytes. Only
                          # meaningful at N = 1: the sharded data-parallel optimizer runs inside the collective phase
                          "optimizer_achieved_gbs": ADAM_BYTES_PER_PARAM * model.n_params / (adam_ms * 1e-3) / 1e9 if (adam_ms > 0 and world == 1) else None,
                          "step_share": fused_ms / ms_per_step if ms_per_step > 0 else None},
@@ -418,12 +408,32 @@ def run_own(args):
         dist.destroy_process_group()
 
 
+DUMP_SAMPLE = 1 << 20  # parameters / gradients per dumped array (fp32: 4 MB each)
+
+
+def dump_outputs(out_dir, model, loss):
+    """The last timed training step's results: loss, updated fp32 parameters and fp16 parameter gradients (as float32). Parameter
+    vectors longer than DUMP_SAMPLE are sampled at fixed, seeded indices (sorted), which are written beside them."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    params = model.trainer.params_full_precision().cpu().numpy().astype(np.float32)
+    grads = model.trainer.param_gradients().cpu().float().numpy().astype(np.float32)
+    n = params.shape[0]
+    idx = np.arange(n, dtype=np.int64) if n <= DUMP_SAMPLE else np.sort(np.random.default_rng(20240611).choice(n, DUMP_SAMPLE, replace=False))
+    np.save(os.path.join(out_dir, "loss.npy"), np.array([loss], dtype=np.float64))
+    np.save(os.path.join(out_dir, "params.npy"), params[idx])
+    np.save(os.path.join(out_dir, "param_gradients.npy"), grads[idx])
+    np.save(os.path.join(out_dir, "sample_indices.npy"), idx.astype(np.float64))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
     ap.add_argument("--steps", type=int, default=200)
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--impl", default="own", choices=["own", "reference"])
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write the last timed step's outputs as DIR/<name>.npy")
     args = ap.parse_args()
     args.warmup = max(3, args.warmup)
     if args.impl == "reference":

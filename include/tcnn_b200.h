@@ -1,4 +1,4 @@
-/* tcnn_b200.h -- C ABI of the Blackwell-native HashGrid + FullyFusedMLP hot path.
+/* tcnn_b200.h -- C ABI of the Hopper-native (sm_90a) HashGrid + FullyFusedMLP hot path.
  *
  * This is the drop-in boundary: plain C, opaque handles, raw device/host pointers, no torch / C++ types.
  * Each entry point names the reference interface (file:line relative to tiny-cuda-nn's tree) it replaces.
@@ -146,7 +146,7 @@ int tcnnb_encoding_backward(tcnnb_encoding* e, tcnnb_stream stream, uint32_t n_e
  * tcnn::create_network<T>(json) (network.h; src/network.cu:51-141; the object benchmarks/mlp/bench_mlp_ours.cu drives) and
  * tcnn::cpp::create_network (cpp_api.h:122; src/cpp_api.cu:160-162 = the same network behind the Identity encoding).
  * `network_json` carries the reference's keys ("otype", "n_neurons", "n_hidden_layers", "activation", "output_activation"); both
- * "FullyFusedMLP" and "CutlassMLP"/"MLP" run on the tcgen05 kernel of csrc/mlp_fused.cu (widths 16/32/64/128, any depth >= 1,
+ * "FullyFusedMLP" and "CutlassMLP"/"MLP" run on the wgmma kernel of csrc/mlp_fused.cu (widths 16/32/64/128, any depth >= 1,
  * padded outputs up to n_neurons). Parameters are CALLER-owned fp16 device arrays (16-byte aligned) in the reference's layout
  * (fully_fused_mlp.cu:635-672): W_0 [n_neurons][input_width], (n_hidden_layers - 1) x [n_neurons][n_neurons],
  * W_out [padded_output_width][n_neurons], row-major; input_width = n_input_dims rounded up to 16.
@@ -170,7 +170,7 @@ int tcnnb_network_forward(tcnnb_network* n, tcnnb_stream stream, uint32_t n_elem
 /* network->backward (Network<T>::backward, fully_fused_mlp.cu:733-866) from what tcnnb_network_forward was given and wrote:
  * dL_doutput fp16 [n][padded_output_width] -> dL_dinput fp16 [n][n_input_dims] and dL_dparams fp16 [n_params] (OVERWRITTEN);
  * either may be null. output_dev is only read when the network has an output activation. Three kernels: the dgrad chain on
- * tcgen05 with the transposed weights read in place (mlp_fused.cu, BWD), the weight-gradient kernel (mlp_wgrad.cu), fp32 -> fp16. */
+ * wgmma with the transposed weights read in place (mlp_fused.cu, BWD), the weight-gradient kernel (mlp_wgrad.cu), fp32 -> fp16. */
 int tcnnb_network_backward(tcnnb_network* n, tcnnb_stream stream, uint32_t n_elements, const void* input_dev, const void* output_dev, const void* hidden_dev,
                            const void* dL_doutput_dev, const void* params_dev, void* dL_dinput_dev, void* dL_dparams_dev);
 /* tcnn::cpp::Module::backward of cpp::create_network (cpp_api.cu:104-125): fp32 input through the Identity encoding; nothing is kept
@@ -183,8 +183,9 @@ int tcnnb_network_inference(tcnnb_network* n, tcnnb_stream stream, uint32_t n_el
 /* The same with the module tier's output convention (cpp_api.cu:82-83): fp16 [n][padded_output_width]. This is what
  * tcnn::cpp::Module::inference / forward of create_network returns. */
 int tcnnb_network_module_inference(tcnnb_network* n, tcnnb_stream stream, uint32_t n_elements, const float* input_dev, void* output_dev, const void* params_dev);
-/* Profiling only (scripts/mlp_timeline.py): clock64 phase stamps of the following launches are written to
- * int64 [n_ctas][5 roles][64 events][8 fields] at clocks_dev (null = off). Not part of the drop-in surface. */
+/* Profiling only: clock64 phase stamps of the following forward / backward-chain launches are written to int64
+ * [n_ctas][5 roles][64 events][8 fields] at clocks_dev (null = off): role = consumer warpgroup (4 unused), event = round * n_steps +
+ * step, fields 0..3 = waiting for the weights / weights ready / product complete / epilogue done. Not part of the drop-in surface. */
 int tcnnb_network_debug_clocks(tcnnb_network* n, void* clocks_dev);
 
 /* ---- data parallelism, natively over NCCL (no counterpart in the single-GPU reference; SURVEY.md section 8e) -------------

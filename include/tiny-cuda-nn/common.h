@@ -25,7 +25,7 @@ namespace tcnn {
 using network_precision_t = __half;                   /* common.h:121-126 (TCNN_HALF_PRECISION builds) */
 static constexpr uint32_t BATCH_SIZE_GRANULARITY = 256; /* common.h:246 */
 static constexpr float LOSS_SCALE = 128.0f;             /* common.h:243 (fp16 parameters) */
-static constexpr uint32_t MIN_GPU_ARCH = 100;           /* this library is sm_100a-only */
+static constexpr uint32_t MIN_GPU_ARCH = 90;            /* this library is sm_90a-only */
 
 enum class MatrixLayout { RowMajor = 0, SoA = 0, ColumnMajor = 1, AoS = 1 }; /* common.h:216-221 */
 static constexpr MatrixLayout RM = MatrixLayout::RowMajor;
@@ -64,7 +64,7 @@ inline void linear_kernel(K kernel, uint32_t shmem_size, cudaStream_t stream, T 
 
 inline int cuda_device() { return tcnnb_cuda_device(); }                 /* common_host.cu:147-151 */
 inline void set_cuda_device(int device) { tcnnb_set_cuda_device(device); }
-inline uint32_t cuda_compute_capability(int = 0) { return 100; }
+inline uint32_t cuda_compute_capability(int = 0) { return 90; }
 inline bool supports_jit_fusion(int = 0) { return false; } /* there is no run-time compilation here: the fused kernel is the product */
 inline void free_all_gpu_memory_arenas() {}                 /* no arenas: nothing is allocated per step */
 

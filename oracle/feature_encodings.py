@@ -4,7 +4,7 @@ TEST INFRASTRUCTURE ONLY (see oracle/README.md): imported by tests/ to check csr
 Each function cites the reference lines it restates. fp32 arithmetic like the kernels (the reference compiles them with
 --use_fast_math, so sin / cos are approximations there: comparisons use a tolerance of a few fp16 ulps, stated in the tests).
 
-Pinned by: tests/golden/composite_*.npz (encoded features dumped from the unmodified reference on a B200, tests/golden/make_golden.sh)
+Pinned by: tests/golden/composite_*.npz (encoded features dumped from the unmodified reference on the GPU, tests/golden/make_golden.sh)
 and, for the spherical harmonics, scipy.special on unit vectors (tests/test_feature_oracle.py).
 """
 import math

@@ -8,7 +8,7 @@
 // replaced by exact (double) sums.
 //
 // Pinning: tests/test_oracle_golden.py checks this file against tests/golden/* (vectors dumped from the
-// reference itself, compiled from /root/reference and run on a B200 by tests/golden/make_golden.sh) and
+// reference itself, compiled from its sources and run on the GPU by tests/golden/make_golden.sh) and
 // against the reference's own known-answer test tests/test_grid.cu:54-71.
 #include "oracle_cpu.h"
 

@@ -19,7 +19,7 @@ enum { ORC_INTERP_NEAREST = 0, ORC_INTERP_LINEAR = 1, ORC_INTERP_SMOOTHSTEP = 2 
 enum { ORC_ACT_RELU = 0, ORC_ACT_LEAKY_RELU = 1, ORC_ACT_SILU = 2, ORC_ACT_EXPONENTIAL = 3, ORC_ACT_SINE = 4, ORC_ACT_SIGMOID = 5,
        ORC_ACT_SQUAREPLUS = 6, ORC_ACT_SOFTPLUS = 7, ORC_ACT_TANH = 8, ORC_ACT_NONE = 9 };  /* common.h:133-144 Activation */
 enum { ORC_LOSS_L2 = 0, ORC_LOSS_RELATIVE_L2 = 1, ORC_LOSS_L1 = 2, ORC_LOSS_RELATIVE_L1 = 3, ORC_LOSS_MAPE = 4, ORC_LOSS_SMAPE = 5, ORC_LOSS_RELATIVE_L2_LUMINANCE = 6, ORC_LOSS_CROSS_ENTROPY = 7, ORC_LOSS_VARIANCE_IS = 8 };  /* src/loss.cu:57-65 */
-enum { ORC_ACCUM_FP32 = 0, ORC_ACCUM_FP16_K16 = 1 };  /* MLP accumulator model: fp32 (tcgen05 path) or fp16 re-rounded every k=16 (HMMA.F16 path) */
+enum { ORC_ACCUM_FP32 = 0, ORC_ACCUM_FP16_K16 = 1 };  /* MLP accumulator model: fp32 (wgmma path) or fp16 re-rounded every k=16 (HMMA.F16 path) */
 
 #define ORC_MAX_LEVELS 128
 

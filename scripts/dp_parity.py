@@ -1,4 +1,4 @@
-"""2-GPU check (run under gpurun --gpus 2 as a plain python script that spawns 2 ranks): data-parallel step == single-GPU step."""
+"""2-GPU check (a plain python script that spawns 2 ranks on a machine with 2 or more GPUs): data-parallel step == single-GPU step."""
 import json
 import os
 import sys
@@ -47,8 +47,9 @@ def worker(rank, world, out, shard_optimizer, native, peer_memory):
 
 
 if __name__ == "__main__":
-    out = os.path.join(ROOT, "gpurun_out")
-    os.makedirs(out, exist_ok=True)
+    import tempfile
+
+    out = tempfile.mkdtemp(prefix="dp_parity_")  # the ranks' parameters and losses, compared below
     # (sharded optimizer, native engine inside libtcnn_b200, peer-memory kernels instead of NCCL collectives)
     MODES = [(False, False, False), (True, False, False), (False, True, False), (True, True, False), (True, True, True)]
     WORLD = int(os.environ.get("TCNNB_DP_WORLD", "2"))

@@ -1,6 +1,6 @@
 // Microbenchmark: throughput of red.global.add.noftz f16x2 reductions of 4 / 8 / 16 bytes at random addresses of a 32 MB table
 // (the access pattern of the hash-grid gradient scatter), as a function of the number of SMs that issue them.
-// Build: nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o red_bench red_bench.cu ; run on the B200 box.
+// Build: nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o red_bench red_bench.cu ; run on an H100.
 #include <cstdint>
 #include <cstdio>
 #include <cuda_runtime.h>
@@ -47,13 +47,13 @@ int main() {
 	const float ghz = khz * 1e-6f;
 	printf("{\"clock_ghz\": %.3f}\n", ghz);
 	for (uint32_t local = 0; local < 2; ++local) {
-		for (int ctas : {8, 37, 74, 148}) {
+		for (int ctas : {8, 33, 66, 132}) {  // up to one CTA per SM of an H100
 			run<1>(table, n - 1, ctas, 512, local, ghz);
 			run<2>(table, n - 1, ctas, 512, local, ghz);
 			run<4>(table, n - 1, ctas, 512, local, ghz);
 		}
 	}
-	run<2>(table, n - 1, 148, 1024, 0, ghz);
-	run<2>(table, n - 1, 296, 512, 0, ghz);
+	run<2>(table, n - 1, 132, 1024, 0, ghz);
+	run<2>(table, n - 1, 264, 512, 0, ghz);
 	return cudaDeviceSynchronize() != cudaSuccess;
 }

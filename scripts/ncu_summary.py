@@ -1,7 +1,7 @@
-"""Turns `ncu --set full` reports into the markdown tables under profiles/ (runs HERE, no GPU: `ncu -i <rep> --page raw --csv`).
+"""Turns `ncu --set full` reports into markdown tables (runs without a GPU: `ncu -i <rep> --page raw --csv`).
 
-    python scripts/ncu_summary.py <title> <report.ncu-rep> [<report2.ncu-rep> ...] > profiles/r02_ncu_summary_<name>.md
-    python scripts/ncu_summary.py --traffic <report.ncu-rep> > profiles/r02_traffic.json
+    python scripts/ncu_summary.py <title> <report.ncu-rep> [<report2.ncu-rep> ...] > ncu_summary_<name>.md
+    python scripts/ncu_summary.py --traffic <report.ncu-rep> > traffic.json
 """
 import csv
 import io
@@ -62,10 +62,10 @@ def main():
             return v * {"Mbyte": 1e6, "Kbyte": 1e3, "Gbyte": 1e9, "byte": 1.0}[units[i]]
 
         print(json.dumps({"kernel": r[hdr.index("Kernel Name")], "dram_bytes_read_per_launch": int(val("dram__bytes_read.sum")), "dram_bytes_write_per_launch": int(val("dram__bytes_write.sum")),
-                          "source": f"ncu --set full --clock-control none ({sys.argv[2].split('/')[-1]}, gpurun, B200); dram__bytes_read.sum + dram__bytes_write.sum"}, indent=1))
+                          "source": f"ncu --set full --clock-control none ({sys.argv[2].split('/')[-1]}); dram__bytes_read.sum + dram__bytes_write.sum"}, indent=1))
         return
     print(f"# {sys.argv[1]}\n")
-    print("Captured on a B200 through gpurun with `ncu --set full --clock-control none --import-source on`; read here with `ncu -i … --page raw --csv`")
+    print("Captured with `ncu --set full --clock-control none --import-source on`; read with `ncu -i … --page raw --csv`")
     print("(scripts/ncu_summary.py). Times under ncu are serialised / cold-cache: bench numbers come from bench.py / scripts/bench_mlp.py only.\n")
     for rep in sys.argv[2:]:
         hdr, units, rows = rows_of(rep)

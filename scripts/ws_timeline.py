@@ -13,8 +13,7 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tiny-cuda-nn_b200"))
-out = os.path.join(ROOT, "gpurun_out", "ws_clocks.bin")
-os.makedirs(os.path.dirname(out), exist_ok=True)
+out = os.path.join(os.environ.get("TCNNB_OUT_DIR", "/tmp"), "ws_clocks.bin")  # phase stamps the library writes (TCNNB_CLOCKS)
 os.environ["TCNNB_CLOCKS"] = out
 os.environ.setdefault("TCNNB_LIB", os.path.join(ROOT, "tiny-cuda-nn_b200", "ablation", "libtcnn_b200.so"))  # the ABLATION=1 build
 import torch
@@ -61,12 +60,10 @@ res = {
         "park": med((mlp[:, steady, 5] - mlp[:, steady, 4]).ravel()),
         # one forward stage (hidden layer 1) and the first backward stage, split up
         "fwd1_stage_sync": med((mlp[:, steady, 7] - mlp[:, steady, 6]).ravel()),
-        "fwd1_mma_issue": med((mlp[:, steady, 8] - mlp[:, steady, 7]).ravel()),
-        "fwd1_mma_wait": med((mlp[:, steady, 9] - mlp[:, steady, 8]).ravel()),
+        "fwd1_mma": med((mlp[:, steady, 9] - mlp[:, steady, 7]).ravel()),  # issue + completion of the wgmma products
         "fwd1_epilogue": med((mlp[:, steady, 10] - mlp[:, steady, 9]).ravel()),
         "bwd1_stage_sync": med((mlp[:, steady, 12] - mlp[:, steady, 11]).ravel()),
-        "bwd1_mma_issue": med((mlp[:, steady, 13] - mlp[:, steady, 12]).ravel()),
-        "bwd1_mma_wait": med((mlp[:, steady, 14] - mlp[:, steady, 13]).ravel()),
+        "bwd1_mma": med((mlp[:, steady, 14] - mlp[:, steady, 12]).ravel()),
         "bwd1_epilogue": med((mlp[:, steady, 15] - mlp[:, steady, 14]).ravel()),
     },
 }

@@ -10,7 +10,7 @@ sys.path.insert(0, ROOT)
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (run with -m gpu on a machine that has one)")
 
 
 @pytest.fixture(scope="session")
@@ -24,6 +24,6 @@ def oracle():
 def torch_cuda():
     import torch
 
-    assert torch.cuda.is_available(), "GPU tests need a B200"
+    assert torch.cuda.is_available(), "GPU tests need an H100"
     torch.cuda.set_device(0)
     return torch

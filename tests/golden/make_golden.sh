@@ -1,8 +1,8 @@
 #!/bin/bash
 # Regenerates tests/golden/<case>/ from the UNMODIFIED reference (oracle/_ref/ref_harness, built by oracle/Makefile from
-# /root/reference). Needs a GPU: run on the B200 box, e.g.
-#   gpurun --timeout 900 -- 'bash tests/golden/make_golden.sh gpurun_out/golden'
-# then copy gpurun_out/golden/<case> into tests/golden/<case> and commit. The vectors are what pins oracle/oracle_cpu.cpp.
+# the reference sources). Needs a GPU: run it on a machine with one, e.g.
+#   bash tests/golden/make_golden.sh <out dir>
+# then pack <out dir>/<case> into tests/golden/<case>.npz (pack_golden.py) and commit. The vectors are what pins oracle/oracle_cpu.cpp.
 set -e
 OUT=${1:-gpurun_out/golden}
 H=oracle/_ref/ref_harness

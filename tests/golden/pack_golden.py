@@ -2,8 +2,8 @@
 """Pack the raw dumps of oracle/ref_harness.cu (gpurun_out/golden/<case>/) into tests/golden/<case>.npz.
 
 Usage: python tests/golden/pack_golden.py gpurun_out/golden tests/golden
-The .npz files are the committed fixtures; they were produced by the unmodified reference (built from /root/reference by
-oracle/Makefile) running on a B200 via tests/golden/make_golden.sh.
+The .npz files are the committed fixtures; they were produced by the unmodified reference (built from its sources by
+oracle/Makefile) running on the GPU via tests/golden/make_golden.sh.
 """
 import glob
 import json

@@ -1,4 +1,4 @@
-"""Loader for tests/golden/*.npz (vectors dumped from the unmodified reference on a B200, see tests/golden/make_golden.sh)."""
+"""Loader for tests/golden/*.npz (vectors dumped from the unmodified reference on the GPU, see tests/golden/make_golden.sh)."""
 import json
 import os
 

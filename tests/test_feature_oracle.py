@@ -1,7 +1,7 @@
 """CPU checks of the numpy oracle of the parameter-free encodings (oracle/feature_encodings.py) -- the checker has to be right before
 the GPU kernels are compared with it: spherical harmonics against scipy on unit vectors, analytic input gradients against central
 differences, OneBlob's partition of unity, Composite's column layout, and -- when the fixtures exist -- the features the unmodified
-reference wrote on a B200 (tests/golden/composite_*.npz)."""
+reference wrote on the GPU (tests/golden/composite_*.npz)."""
 import os
 import sys
 

@@ -1,5 +1,5 @@
 """BASELINE.json configs[0] as a path of this library: Identity encoding (encodings/identity.h:46-67) + a 64 x 2 network
-("CutlassMLP" / "MLP" / "FullyFusedMLP" all run on the tcgen05 kernels) through create_from_config / trainer->training_step.
+("CutlassMLP" / "MLP" / "FullyFusedMLP" all run on the wgmma kernels) through create_from_config / trainer->training_step.
 Checked against the oracle's MLP stage functions fed with the Identity features, and -- when tests/golden/identity_cutlass.npz
 exists -- against vectors dumped by the unmodified reference (its CutlassMLP path, cutlass_mlp.cu:272-308)."""
 import ctypes

@@ -1,5 +1,5 @@
-"""GPU parity of the stand-alone FullyFusedMLP kernel (csrc/mlp_fused.cu: TMA-staged weights, activations threaded through tensor
-memory, A-from-TMEM tcgen05.mma) against the CPU oracle's restatement of kernel_mlp_fused (oracle_cpu.cpp orc_mlp_forward,
+"""GPU parity of the stand-alone FullyFusedMLP kernel (csrc/mlp_fused.cu: TMA-staged weights, activations threaded through
+registers as the A operand of wgmma) against the CPU oracle's restatement of kernel_mlp_fused (oracle_cpu.cpp orc_mlp_forward,
 fully_fused_mlp.cu:499-557), through the C ABI's network tier (tcnnb_network_*)."""
 import ctypes
 
@@ -136,9 +136,9 @@ MLP_GOLDEN = sorted(os.path.splitext(os.path.basename(p))[0] for p in glob.glob(
 @pytest.mark.parametrize("name", MLP_GOLDEN)
 def test_network_against_reference_golden_vectors(torch_cuda, name):
     """tests/golden/mlp_*.npz: weights, fp16 inputs and fp16 outputs of the UNMODIFIED reference's Network<__half>::inference_mixed_precision
-    (`ref_harness mlpdump`: create_network<T>(json), FullyFusedMLP 128 x 4 / 64 x 2 / 32 x 3 Tanh->Sigmoid, CutlassMLP 64 x 2) on a B200.
+    (`ref_harness mlpdump`: create_network<T>(json), FullyFusedMLP 128 x 4 / 64 x 2 / 32 x 3 Tanh->Sigmoid, CutlassMLP 64 x 2) on the GPU.
     Same weights, same inputs -> outputs within the reference's own forward bar (tests/test_common.h:177: RAE < 1e-2 @ p99); the
-    difference is the accumulator: fp16 inside HMMA there, fp32 in tensor memory here."""
+    difference is the accumulator: fp16 inside HMMA there, fp32 in registers (wgmma) here."""
     torch = torch_cuda
     import tcnn_b200
 

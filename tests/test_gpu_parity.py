@@ -1,4 +1,4 @@
-"""GPU parity tests: every stage of the fused sm_100a kernel against the CPU oracle on identical seeded inputs, through
+"""GPU parity tests: every stage of the fused sm_90a kernel against the CPU oracle on identical seeded inputs, through
 the C ABI (libtcnn_b200.so). Integer work (cells, hash indices => which table entries are blended) must be bit-exact,
 which shows up as bit-exact encoded features; floating-point stages are checked stage-by-stage (each oracle stage is fed
 the DEVICE's previous stage) within stated fp16 tolerances, using the reference's own vocabulary (tests/test_common.h:59-117:
@@ -93,7 +93,7 @@ def test_stagewise_parity(torch_cuda, name, n_in, n_out, B):
     assert np.array_equal(enc_dev[:, :W].T, enc_ref), "encoded features differ"
     assert (enc_dev[:, W:] == 0).all()
 
-    # ---- stage 2: MLP forward on the device's encoding (oracle with fp32 accumulation like tcgen05)
+    # ---- stage 2: MLP forward on the device's encoding (oracle with fp32 accumulation like wgmma)
     hid_ref, out_ref = orc.mlp_forward(np.ascontiguousarray(enc_dev[:, :W].T))
     hid_dev = f16(taps["hidden"])
     a, b = ob.half_bits_to_float(hid_dev), ob.half_bits_to_float(hid_ref)
@@ -281,7 +281,7 @@ def test_errors_fail_loudly(torch_cuda):
 
 
 # ------------------------------------------------------------------------------------------------------------------
-# Against the reference itself: tests/golden/*.npz were dumped by the UNMODIFIED reference (sm_100 build) on a B200.
+# Against the reference itself: tests/golden/*.npz were dumped by the UNMODIFIED reference (its own GPU build).
 # ------------------------------------------------------------------------------------------------------------------
 from golden_util import CASES as GOLDEN_CASES, load_case, load_config, mlp_gradients_agree  # noqa: E402
 
@@ -328,7 +328,7 @@ def test_against_reference_golden_vectors(torch_cuda, name):
     ref = ob.half_bits_to_float(g["grads_step0_f16"])
     n_mlp = model.n_mlp_params
     # The MLP weight gradients are where the accumulator model matters: the reference accumulates 512..2^18 products in
-    # fp16 (CUTLASS split-K, cutlass_matmul.h:67), this kernel in fp32 (tcgen05). The reference's own two implementations
+    # fp16 (CUTLASS split-K, cutlass_matmul.h:67), this kernel in fp32 (wgmma). The reference's own two implementations
     # (offline vs JIT) differ by 1.17e-2 on this vector, the fp32-accumulating oracle sits 1.23e-2 / 1.34e-2 from them and
     # the fp16-accumulating oracle 7e-4 from the offline kernels (tests/test_oracle_golden.py): bar = 2e-2 for the MLP part.
     assert mlp_gradients_agree(grads[:n_mlp], ref[:n_mlp], 2e-2)

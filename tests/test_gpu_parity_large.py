@@ -92,7 +92,7 @@ def test_benchmarked_size_against_reference(torch_cuda, name):
     grads = ob.half_bits_to_float(f16(model.trainer.param_gradients()))
     gs = param_sample(grads, n_net, stride)
     ref = ob.half_bits_to_float(g["grads_step0_f16"])
-    # network weight gradients: fp32 (tcgen05) vs fp16 split-K accumulation in the reference -> the relaxed 2e-2 bar, this row only
+    # network weight gradients: fp32 (wgmma) vs fp16 split-K accumulation in the reference -> the relaxed 2e-2 bar, this row only
     assert mlp_gradients_agree(gs[:n_net], ref[:n_net], 2e-2)
     # Grid gradients. At these batch sizes every coarse entry receives hundreds of fp16 atomic addends and the REFERENCE's result is
     # itself 1-2e-2 (RAE) away from the exact sums (`grads_exact_f32`: the oracle's double-accumulated sums, added to the fixture by
@@ -129,7 +129,7 @@ def test_benchmarked_size_against_reference(torch_cuda, name):
 
 
 def test_multi_tile_binned_kernel_matches_oracle(torch_cuda):
-    """65 536 samples of the headline configuration (T = 2^19): 512 tiles on 148 persistent CTAs -> 3-4 tiles per CTA, binning on.
+    """65 536 samples of the headline configuration (T = 2^19): 512 tiles on 132 persistent CTAs (H100) -> 3-4 tiles per CTA, binning on.
     Every sample's encoding is bit-exact with the oracle; gradients within the reference's bars of the oracle's exact sums; the
     binned and the unbinned step touch exactly the same table entries."""
     torch = torch_cuda

@@ -1,5 +1,5 @@
 """Pins oracle/oracle_cpu.cpp against the reference itself: vectors dumped by the UNMODIFIED reference (compiled from
-/root/reference, run on a B200) and committed under tests/golden/. Integer/bit-level quantities must match exactly;
+the reference sources, run on the GPU) and committed under tests/golden/. Integer/bit-level quantities must match exactly;
 floating-point stages are held to the reference's own test tolerances (tests/test_common.h:153-219). CPU only."""
 import numpy as np
 import pytest

@@ -7,7 +7,7 @@
 // in L1) instead of 32 different ones. Gradients and the loss are sums over samples, so processing the batch in a different
 // order changes nothing but the (already unordered) accumulation order; per-sample outputs are written through `perm`.
 //
-// The reference has no counterpart (it consumes the batch in the caller's order); this is a B200-specific scheduling step.
+// The reference has no counterpart (it consumes the batch in the caller's order); this is a scheduling step of this library.
 #include "binning.h"
 
 namespace tcnnb {

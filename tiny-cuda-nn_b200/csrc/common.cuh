@@ -9,7 +9,7 @@ namespace tcnnb {
 
 constexpr uint32_t MAX_LEVELS = 32;            // levels handled by the by-value kernel argument (L*F <= 64 on the fused path)
 constexpr uint32_t BATCH_GRANULARITY = 256;    // common.h:246 BATCH_SIZE_GRANULARITY
-constexpr uint32_t TILE_M = 128;               // samples per MMA tile = TMEM lanes
+constexpr uint32_t TILE_M = 128;               // samples per MMA tile (two m64 wgmma products)
 
 // Same numeric values as the reference enums (common.h:133-164).
 enum Activation : uint32_t { ACT_RELU = 0, ACT_LEAKY_RELU = 1, ACT_SILU = 2, ACT_EXPONENTIAL = 3, ACT_SINE = 4, ACT_SIGMOID = 5, ACT_SQUAREPLUS = 6, ACT_SOFTPLUS = 7, ACT_TANH = 8, ACT_NONE = 9 };

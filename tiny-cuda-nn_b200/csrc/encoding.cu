@@ -37,7 +37,7 @@ static void build_encoding(Encoding& e, uint32_t n_input_dims, const json::Value
 	TCNNB_CUDA_CHECK(cudaGetDevice(&device));
 	cudaDeviceProp prop;
 	TCNNB_CUDA_CHECK(cudaGetDeviceProperties(&prop, device));
-	if (prop.major != 10) throw std::runtime_error("tcnn_b200 requires an sm_100-class GPU (B200); found compute capability " + std::to_string(prop.major) + "." + std::to_string(prop.minor));
+	if (prop.major != 9) throw std::runtime_error("tcnn_b200 requires an sm_90-class GPU (H100); found compute capability " + std::to_string(prop.major) + "." + std::to_string(prop.minor));
 	e.scratch.resize(128);
 	build_encoding_plan(e.plan, n_input_dims, cfg, 0, e.scratch.ptr);
 	for (auto& g : e.plan.grids) {

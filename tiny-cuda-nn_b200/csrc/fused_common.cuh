@@ -1,4 +1,4 @@
-// fused_common.cuh -- device helpers shared by the tcgen05 kernels (fused_ws.cu, mlp_fused.cu).
+// fused_common.cuh -- device helpers shared by the wgmma kernels (fused_ws.cu, mlp_fused.cu).
 #pragma once
 #include "common.cuh"
 #include "ptx.cuh"

@@ -52,6 +52,19 @@ struct FusedStepParams {
 	long long* dbg_clock;          // ablation builds: [cta][role 3][tile 16][slot 16] clock64 stamps of the ws kernel's phases
 };
 
+// Shared memory of the fused kernel: encoded / hidden / dy tiles of 128 x 64 fp16 (an encoding of at most 32 features parks its
+// gradients in the enc tiles, wider ones need two park tiles), the staged weights, and the barriers ...
+__host__ __device__ inline uint32_t fused_ws_base_smem_bytes(uint32_t n_hidden_layers, uint32_t enc_width, bool train) {
+	const uint32_t tiles = 2 + n_hidden_layers + (train ? (enc_width <= 32 ? 1 : 3) : 0);
+	return tiles * TILE_M * 128 + n_hidden_layers * 64 * 128 + 16 * 128 + 128;
+}
+// ... and, in training, the CTA's fp32 weight-gradient sums ([64 x 64] per hidden-layer input matrix, [64 x 16] for the output
+// matrix) when they fit beside it. Deeper networks add each tile's weight gradients to the global accumulator instead.
+__host__ __device__ inline uint32_t fused_ws_dw_bytes(uint32_t n_hidden_layers) { return n_hidden_layers * 64 * 64 * 4 + 64 * 16 * 4; }
+__host__ __device__ inline bool fused_ws_dw_in_smem(uint32_t n_hidden_layers, uint32_t enc_width) {
+	return fused_ws_base_smem_bytes(n_hidden_layers, enc_width, true) + fused_ws_dw_bytes(n_hidden_layers) <= 227 * 1024;
+}
+
 // Warp-specialised kernel (fused_ws.cu): one 640-thread CTA per SM (n_ctas <= #SMs), training step and inference.
 size_t fused_ws_smem_bytes(uint32_t n_hidden_layers, uint32_t enc_width, bool train);
 cudaError_t launch_fused_ws(const FusedStepParams& p, uint32_t n_pos_dims, bool train, uint32_t n_ctas, cudaStream_t stream);

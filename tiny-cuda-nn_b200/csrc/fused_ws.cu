@@ -1,5 +1,5 @@
-// fused_ws.cu -- the hot path in ONE warp-specialised kernel: HashGrid gather + N-linear blend -> FullyFusedMLP forward (tcgen05)
-// -> loss -> MLP backward (tcgen05: dgrad and wgrad) -> hash-grid gradient scatter (f16x2 reductions); without its backward half
+// fused_ws.cu -- the hot path in ONE warp-specialised kernel: HashGrid gather + N-linear blend -> FullyFusedMLP forward (wgmma)
+// -> loss -> MLP backward (wgmma: dgrad and wgrad) -> hash-grid gradient scatter (f16x2 reductions); without its backward half
 // it is the inference kernel.
 //
 // Replaces, for one training step, the reference's kernel_grid (grid.h:49), kernel_mlp_fused (fully_fused_mlp.cu:500),
@@ -12,29 +12,24 @@
 // a K-major A operand by the forward / dgrad MMAs (M = samples, K = neurons) and as an MN-major operand by the wgrad MMAs
 // (M/N = neurons, K = samples), so no transposes are ever materialised. Weights are staged once per CTA: W_l [out][in] row-major
 // is the K-major B operand of the forward MMA and, read MN-major, the B operand of the dgrad MMA (W_l^T). Accumulators live in
-// TMEM: ACC (64 columns, reused by every layer) + one 64x64 fp32 wgrad accumulator per weight matrix that persists across all
-// tiles of the CTA and is flushed once with red.global.add.f32. The backward activations g_l overwrite h_l in place.
+// the MLP warpgroup's registers; the fp32 weight-gradient sums of all tiles of the CTA live in shared memory (when they fit, see
+// fused_ws_dw_in_smem) and are flushed once with red.global.add.f32. The backward activations g_l overwrite h_l in place.
 //
-// Why warp-specialised: in a bulk-synchronous structure (round 1's fused_step.cu, removed) every MMA batch ends in a CTA-wide
-// barrier, so the long and uneven latencies of the table gathers / gradient reductions that fill the wait slots end up on the
-// critical path of the MLP chain (12 % barrier stalls, 45 % long-scoreboard; 25 % slower for training, 43 % for inference).
+// Why warp-specialised: in a bulk-synchronous structure every MMA batch ends in a CTA-wide barrier, so the long and uneven
+// latencies of the table gathers / gradient reductions that fill the wait slots end up on the critical path of the MLP chain.
 // Here the two kinds of work never wait for each other inside a tile:
 //
-//   warps 0..3   "MLP group" (128 threads, thread t <-> tile row t <-> TMEM lane t): issues the tcgen05 MMAs and runs the
-//                epilogues of one 128-sample tile at a time, tile after tile.
+//   warps 0..3   "MLP group" (one warpgroup): issues the wgmma products and runs the epilogues of one 128-sample tile at a time,
+//                tile after tile.
 //   warps 4..19  "memory group": two sub-groups of 8 warps (256 threads = two threads per sample). Sub-group g owns the
 //                tiles k = g, g+2, ... of this CTA: it gathers + blends tile k into enc[g], then scatters the parked
 //                dL/d(enc) of its previous tile k-2, continuously, while the MLP group works on tile k-1.
-//                (Running two MLP chains ping-pong in the MLP group was tried and is SLOWER -- it phase-locks the two
-//                memory sub-groups; scripts/experiments/fused_ws_dual_chain.cu.txt, DESIGN.md section 5.)
 //
 // Hand-offs are mbarriers only:  enc_full[g]  (memory -> MLP: encoded tile ready)
-//                                enc_free[g]  (tcgen05.commit -> memory: last MMA that reads enc[g] has finished)
+//                                enc_free[g]  (MLP -> memory: the last wgmma that reads enc[g] has completed)
 //                                park_full[g] (MLP -> memory: dL/d(enc) of the tile parked)
 //                                park_free[g] (memory -> MLP: parked gradients consumed)
-// One persistent CTA per SM, 640 threads (4 MLP warps + two memory sub-groups), grid = #SMs. (A second shape -- two 384-thread
-// CTAs per SM with one memory sub-group each -- was measured slower, 0.265 vs 0.213 ms on the headline configuration, and
-// was removed; DESIGN.md section 3.1 keeps the number.)
+// One persistent CTA per SM, 640 threads (4 MLP warps + two memory sub-groups), grid = #SMs.
 #include "common.cuh"
 #include "fused_common.cuh"
 #include "fused_step.h"
@@ -67,6 +62,7 @@ constexpr uint32_t WS_MLP_THREADS = 128;
 constexpr uint32_t WS_SUB_THREADS = 256;
 constexpr uint32_t SUBS = 2;  // memory sub-groups per CTA
 constexpr uint32_t WS_THREADS = WS_MLP_THREADS + SUBS * WS_SUB_THREADS;  // 640
+constexpr uint32_t WS_DW_BYTES = 64 * 64 * 4;  // fp32 weight-gradient sums of one hidden-layer input matrix
 
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
 	asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
@@ -110,20 +106,22 @@ __global__ void __launch_bounds__(WS_THREADS, 1) fused_ws_kernel(const FusedStep
 		return park_in_enc ? s_enc + g * TILE_BYTES + sw128(row, 4u + chunk) : s_park + g * TILE_BYTES + sw128(row, chunk);
 	};
 	const uint32_t s_wout = s_w0 + NH * (WIDTH * 128);
-	const uint32_t s_bars = s_wout + 16 * 128;  // 9 mbarriers
-	const uint32_t bar_mma = s_bars;
+	// fp32 weight-gradient sums of this CTA (training, when they fit: fused_ws_dw_in_smem): one [64 x 64] block per hidden-layer input
+	// matrix W_0 .. W_{NH-1} and one [64 x 16] block for W_out, kept across all tiles. Stored in the accumulator fragment order of
+	// the MLP warpgroup -- word (i * 128 + thread) * 4 + q holds d[4 i + q] of that thread -- so that every thread reloads and
+	// stores only its own values.
+	const bool dw_smem = TRAIN && fused_ws_dw_in_smem(NH, in_w);
+	const uint32_t s_dw = s_wout + 16 * 128;
+	const uint32_t s_bars = s_dw + (dw_smem ? fused_ws_dw_bytes(NH) : 0);  // 9 mbarriers
 	const uint32_t bar_enc_full = s_bars + 8;    // [4]
 	const uint32_t bar_enc_free = s_bars + 40;   // [4]
 	const uint32_t bar_park_full = s_bars + 72;  // [2]
 	const uint32_t bar_park_free = s_bars + 88;  // [2]
-	const uint32_t s_tmem_slot = s_bars + 104;
 
-	const uint32_t tmem_cols = TRAIN ? ((NH + 2) * 64 <= 256 ? 256u : 512u) : 64u;
 	if (tid == 0) {
-		mbar_init(bar_mma, 1);
 		for (uint32_t e = 0; e < NE; ++e) {
 			mbar_init(bar_enc_full + 8 * e, WS_SUB_THREADS / 32);   // one arrival per memory warp
-			mbar_init(bar_enc_free + 8 * e, 1);                      // tcgen05.commit
+			mbar_init(bar_enc_free + 8 * e, WS_MLP_THREADS / 32);   // one arrival per MLP warp once its last wgmma reading enc completed
 		}
 		for (uint32_t g = 0; g < 2; ++g) {
 			mbar_init(bar_park_full + 8 * g, WS_MLP_THREADS / 32);  // one arrival per MLP warp
@@ -131,13 +129,11 @@ __global__ void __launch_bounds__(WS_THREADS, 1) fused_ws_kernel(const FusedStep
 		}
 		fence_mbar_init();
 	}
-	if (warp == 0) {
-		__syncwarp();
-		tmem_alloc(s_tmem_slot, tmem_cols);
-		tmem_relinquish();
+	if (dw_smem) {
+		for (uint32_t i = tid; i < fused_ws_dw_bytes(NH) / 16; i += WS_THREADS) st_shared_v4(s_dw + 16 * i, 0, 0, 0, 0);
 	}
 
-	pdl_wait();  // everything above touched only shared / tensor memory; from here on the previous kernel's writes are needed
+	pdl_wait();  // everything above touched only shared memory; from here on the previous kernel's writes are needed
 	{
 		// W_l [out][in] row-major -> 128-byte tile rows (K-major, SWIZZLE_128B). Rows / columns beyond the network's width
 		// and the encoding's width are zero, which makes a 16- or 32-wide network an exact sub-problem of the 64-wide tiles.
@@ -160,22 +156,21 @@ __global__ void __launch_bounds__(WS_THREADS, 1) fused_ws_kernel(const FusedStep
 		stage(s_wout, w, 16, NW, 16);
 	}
 	fence_proxy_async_smem();
-	tc_fence_before_sync();
 	__syncthreads();
-	tc_fence_after_sync();
 
-	uint32_t tmem_base;
-	asm volatile("ld.shared.b32 %0, [%1];" : "=r"(tmem_base) : "r"(s_tmem_slot));
 	const uint32_t n_tiles = p.batch_size / TILE_M;
-	// Tiles of this CTA: a CONTIGUOUS range [cta_first, cta_end) of the (spatially binned) batch. With the round-robin assignment of
-	// round 1 (tile = blockIdx + k * gridDim) all 148 CTAs worked on 148 neighbouring tiles at any moment, i.e. on the same few
-	// cells of the coarse dense levels, and their reductions queued up on the same L2 addresses (ablation: the 4 dense levels -- a
-	// quarter of the reductions -- cost 0.047 of the kernel's 0.217 ms). Contiguous ranges put concurrent CTAs in different regions.
+	// Tiles of this CTA: a CONTIGUOUS range [cta_first, cta_end) of the (spatially binned) batch. With a round-robin assignment
+	// (tile = blockIdx + k * gridDim) all CTAs work on neighbouring tiles at any moment, i.e. on the same few cells of the coarse
+	// dense levels, and their reductions queue up on the same L2 addresses. Contiguous ranges put concurrent CTAs in different regions.
 	const uint32_t cta_first = (uint32_t)(((uint64_t)blockIdx.x * n_tiles) / gridDim.x);
 	const uint32_t cta_end = (uint32_t)(((uint64_t)(blockIdx.x + 1) * n_tiles) / gridDim.x);
 
 	if (warp >= WS_MLP_THREADS / 32) {
 		// =========================================================================================== memory group
+		// 640 threads start with 96 registers each (the count ptxas reports for the kernel); the MLP warpgroup holds two 64-column
+		// accumulator fragments and takes what the memory warps give up (512 x 80 + 128 x 160 = 640 x 96). ptxas allocates each
+		// branch to its new limit: without the exchange the training variants spill several hundred bytes.
+		asm volatile("setmaxnreg.dec.sync.aligned.u32 80;\n" ::: "memory");
 		const uint32_t mt = tid - WS_MLP_THREADS;
 		const uint32_t sub = mt / WS_SUB_THREADS;   // sub-group; with SUBS == 2 it owns the tiles (and buffers) of parity `sub`
 		const uint32_t lt = mt % WS_SUB_THREADS;
@@ -340,7 +335,7 @@ __global__ void __launch_bounds__(WS_THREADS, 1) fused_ws_kernel(const FusedStep
 					}
 				}
 			}
-			fence_proxy_async_smem();  // the tile is read by tcgen05.mma (async proxy)
+			fence_proxy_async_smem();  // the tile is read by wgmma (async proxy)
 			__syncwarp();
 			if ((tid & 31u) == 0) mbar_arrive(bar_enc_full + 8 * e);
 			if (lt == 0) WS_STAMP(1 + sub, k, 2);
@@ -368,29 +363,92 @@ __global__ void __launch_bounds__(WS_THREADS, 1) fused_ws_kernel(const FusedStep
 		}
 	} else {
 		// =========================================================================================== MLP group
+		// One warpgroup. Every MMA covers the 128-row tile as two m64 halves; thread (warp w, lane) holds the accumulator fragment
+		// rows mh * 64 + 16 w + lane / 4 (+ 8), columns 8 i + 2 (lane % 4) (+ 1) -- see Wgmma in ptx.cuh. The per-row work of the
+		// output layer (loss, outputs) is done by thread `row` after the fragment has been staged in shared memory.
+		asm volatile("setmaxnreg.inc.sync.aligned.u32 160;\n" ::: "memory");
 		const uint32_t row = tid;  // 0..127
-		const uint32_t lane_field = (warp * 32u) << 16;
-		const uint32_t tmem_acc = tmem_base;
-		uint32_t phase = 0;
+		const uint32_t fq = (tid & 31u) >> 2, ft = tid & 3u;
 		float loss_acc = 0.0f;
 		bool dw_started = false;
+		auto frow = [&](uint32_t mh, uint32_t hi) { return mh * 64u + warp * 16u + fq + hi * 8u; };
 
-		constexpr uint32_t IDESC_FWD_N64 = umma_idesc_f16(128, 64, 0, 0);
-		constexpr uint32_t IDESC_FWD_N16 = umma_idesc_f16(128, 16, 0, 0);
-		constexpr uint32_t IDESC_DGRAD = umma_idesc_f16(128, 64, 0, 1);
-		constexpr uint32_t IDESC_WGRAD = umma_idesc_f16(64, 64, 1, 1);
-		auto kmaj = [](uint32_t tile, uint32_t jj) { return umma_desc_sw128(tile + jj * 32u, 16u, 1024u); };
-		auto mnmaj = [](uint32_t tile, uint32_t jj) { return umma_desc_sw128(tile + jj * 2048u, TILE_BYTES, 1024u); };
+		auto kmaj = [](uint32_t tile, uint32_t jj) { return wgmma_desc_sw128(tile + jj * 32u, 16u, 1024u); };
+		auto mnmaj = [](uint32_t tile, uint32_t jj) { return wgmma_desc_sw128(tile + jj * 2048u, TILE_BYTES, 1024u); };
 		auto stage_sync = [&]() {
-			tmem_ld_wait();
-			tc_fence_before_sync();
 			fence_proxy_async_smem();
 			named_bar_sync(1, WS_MLP_THREADS);
 		};
-		auto wait_mma = [&]() {
-			mbar_wait(bar_mma, phase);
-			phase ^= 1u;
-			tc_fence_after_sync();
+		// this warp's wgmma groups have completed: release an mbarrier that counts one arrival per MLP warp
+		auto warp_arrive = [&](uint32_t bar) {
+			__syncwarp();
+			if ((tid & 31u) == 0) mbar_arrive(bar);
+		};
+		// acc[mh] = A[rows of half mh] . B over `ksteps` steps of 16: A K-major (128-row tile), B K-major (forward) or MN-major (dgrad)
+		float acc[2][32];
+		auto mma64 = [&](uint32_t a_tile, uint32_t b_tile, uint32_t ksteps, bool b_mn) {
+			wgmma_fence();
+#pragma unroll
+			for (uint32_t mh = 0; mh < 2; ++mh) {
+				for (uint32_t jj = 0; jj < ksteps; ++jj) {
+					if (b_mn) Wgmma<64>::ss<0, 1>(acc[mh], kmaj(a_tile + mh * 8192u, jj), mnmaj(b_tile, jj), jj > 0);
+					else Wgmma<64>::ss<0, 0>(acc[mh], kmaj(a_tile + mh * 8192u, jj), kmaj(b_tile, jj), jj > 0);
+				}
+			}
+			wgmma_commit();
+			wgmma_wait<0>();
+			reg_fence(acc[0]);
+			reg_fence(acc[1]);
+		};
+		// fragment words d[4 i .. 4 i + 3] of weight matrix l (l == NH: W_out) -> the global fp32 accumulator. d[4 i + q]: row
+		// m = 16 w + lane / 4 (+ 8 for q >= 2), column n = 8 i + 2 (lane % 4) + (q & 1); the rows are the matrix's outputs, for W_out its inputs
+		auto flush_dw = [&](uint32_t l, uint32_t i, const float* x) {
+			const uint32_t n = 8 * i + 2 * ft;
+#pragma unroll
+			for (uint32_t hi = 0; hi < 2; ++hi) {
+				const uint32_t m = warp * 16 + fq + hi * 8;
+				const float v0 = x[2 * hi], v1 = x[2 * hi + 1];
+				if (m >= p.width) continue;
+				if (l == 0) {
+					if (n < in_w) red_add_v2_f32(p.dw_accum + m * in_w + n, v0, v1);
+				} else if (l < NH) {
+					if (n < p.width) red_add_v2_f32(p.dw_accum + p.width * in_w + (l - 1) * p.width * p.width + m * p.width + n, v0, v1);
+				} else {
+					float* dst = p.dw_accum + p.width * in_w + (NH - 1) * p.width * p.width;  // W_out [16][width]
+					red_add_f32(dst + n * p.width + m, v0);
+					red_add_f32(dst + (n + 1) * p.width + m, v1);
+				}
+			}
+		};
+		// dW_l += A^T . B over the tile's 128 samples (both operands MN-major): N = 64, or 16 for W_out (l == NH). The fp32 sums
+		// round-trip through s_dw, or go to the global accumulator after every tile.
+		auto wgrad = [&](uint32_t l, uint32_t a_tile, uint32_t b_tile) {
+			const uint32_t dw_addr = s_dw + l * WS_DW_BYTES;
+			const uint32_t n_i = l == NH ? 2u : 8u;
+			float d[32];
+#pragma unroll
+			for (uint32_t i = 0; i < 8; ++i) {
+				uint32_t x = 0, y = 0, z = 0, w = 0;
+				if (dw_smem && i < n_i) ld_shared_v4(dw_addr + (i * WS_MLP_THREADS + tid) * 16u, x, y, z, w);
+				d[4 * i] = __uint_as_float(x), d[4 * i + 1] = __uint_as_float(y), d[4 * i + 2] = __uint_as_float(z), d[4 * i + 3] = __uint_as_float(w);
+			}
+			wgmma_fence();
+			if (l == NH) {
+#pragma unroll
+				for (uint32_t jj = 0; jj < TILE_M / 16; ++jj) Wgmma<16>::ss<1, 1>(reinterpret_cast<float(&)[8]>(d[0]), mnmaj(a_tile, jj), mnmaj(b_tile, jj), 1);
+			} else {
+#pragma unroll
+				for (uint32_t jj = 0; jj < TILE_M / 16; ++jj) Wgmma<64>::ss<1, 1>(d, mnmaj(a_tile, jj), mnmaj(b_tile, jj), 1);
+			}
+			wgmma_commit();
+			wgmma_wait<0>();
+			reg_fence(d);
+#pragma unroll
+			for (uint32_t i = 0; i < 8; ++i) {
+				if (i >= n_i) continue;
+				if (dw_smem) st_shared_v4(dw_addr + (i * WS_MLP_THREADS + tid) * 16u, __float_as_uint(d[4 * i]), __float_as_uint(d[4 * i + 1]), __float_as_uint(d[4 * i + 2]), __float_as_uint(d[4 * i + 3]));
+				else flush_dw(l, i, d + 4 * i);
+			}
 		};
 
 		const uint32_t n_batches = TRAIN ? 2 * NH + 2 : NH + 1;
@@ -398,11 +456,11 @@ __global__ void __launch_bounds__(WS_THREADS, 1) fused_ws_kernel(const FusedStep
 		// group's traffic, would otherwise sit in the middle of this group's dependent MMA / epilogue chain: the index is
 		// fetched one tile ahead, the targets at the top of the tile (the loss needs them three MMA stages later).
 		constexpr uint32_t N_TGT_PREFETCH = 4;
-		auto sample_of = [&](uint32_t tile) {
-			const uint32_t s = tile * TILE_M + row;
+		auto sample_of = [&](uint32_t tile, uint32_t r) {
+			const uint32_t s = tile * TILE_M + r;
 			return p.perm ? __ldg(p.perm + s) : s;
 		};
-		uint32_t osample_next = cta_first < cta_end ? sample_of(cta_first) : 0;
+		uint32_t osample_next = cta_first < cta_end ? sample_of(cta_first, row) : 0;
 		uint32_t k = 0;
 		for (uint32_t tile = cta_first; tile < cta_end; ++tile, ++k) {
 			const uint32_t g = k & 1u, j = k >> 1;
@@ -420,7 +478,7 @@ __global__ void __launch_bounds__(WS_THREADS, 1) fused_ws_kernel(const FusedStep
 					for (uint32_t q = 0; q < N_TGT_PREFETCH; ++q) tgt[q] = q < p.n_out ? __ldg(p.targets + (size_t)osample * p.n_out + q) : 0.0f;
 				}
 			}
-			if (tile + 1 < cta_end) osample_next = sample_of(tile + 1);
+			if (tile + 1 < cta_end) osample_next = sample_of(tile + 1, row);
 			if (tid == 0) WS_STAMP(0, k, 0);
 			mbar_wait(bar_enc_full + 8 * e, je & 1u);
 			if (tid == 0) WS_STAMP(0, k, 1);
@@ -432,71 +490,86 @@ __global__ void __launch_bounds__(WS_THREADS, 1) fused_ws_kernel(const FusedStep
 				stage_sync();
 				if (tid == 0 && b == NH + 1) WS_STAMP(0, k, 2);
 				if (tid == 0 && (b == 1 || b == NH + 1)) WS_STAMP(0, k, b == 1 ? 7 : 12);
-				if (warp == 0 && elect_one_sync()) {  // warp-uniform branch + one elected lane: operands stay in uniform registers
-					tc_fence_after_sync();
-					if (b < NH) {
-						const uint32_t a_tile = b == 0 ? enc_cur : s_h0 + (b - 1) * TILE_BYTES;
-						const uint32_t b_tile = s_w0 + b * (WIDTH * 128);
-						const uint32_t ksteps = b == 0 ? in_w / 16 : WIDTH / 16;
-						for (uint32_t jj = 0; jj < ksteps; ++jj) umma_f16_ss(tmem_acc, kmaj(a_tile, jj), kmaj(b_tile, jj), IDESC_FWD_N64, jj > 0);
-						if (!TRAIN && b == 0) umma_commit(bar_enc_free + 8 * e);  // inference: L0 is the only reader of enc
-					} else if (b == NH) {
-						const uint32_t a_tile = s_h0 + (NH - 1) * TILE_BYTES;
-						for (uint32_t jj = 0; jj < WIDTH / 16; ++jj) umma_f16_ss(tmem_acc, kmaj(a_tile, jj), kmaj(s_wout, jj), IDESC_FWD_N16, jj > 0);
-					} else if (b <= 2 * NH) {
-						const uint32_t l = 2 * NH + 1 - b;
-						const uint32_t h_prev = s_h0 + (l - 1) * TILE_BYTES;
-						if (l == NH) {
-							umma_f16_ss(tmem_acc, kmaj(s_dy, 0), mnmaj(s_wout, 0), IDESC_DGRAD, 0);
-							const uint32_t dw = tmem_base + 64u * (1 + NH);
-							for (uint32_t jj = 0; jj < TILE_M / 16; ++jj) umma_f16_ss(dw, mnmaj(h_prev, jj), mnmaj(s_dy, jj), IDESC_WGRAD, dw_started || jj > 0);
-						} else {
-							const uint32_t g_tile = s_h0 + l * TILE_BYTES;
-							const uint32_t w_tile = s_w0 + l * (WIDTH * 128);
-							for (uint32_t jj = 0; jj < WIDTH / 16; ++jj) umma_f16_ss(tmem_acc, kmaj(g_tile, jj), mnmaj(w_tile, jj), IDESC_DGRAD, jj > 0);
-							const uint32_t dw = tmem_base + 64u * (1 + l);
-							for (uint32_t jj = 0; jj < TILE_M / 16; ++jj) umma_f16_ss(dw, mnmaj(g_tile, jj), mnmaj(h_prev, jj), IDESC_WGRAD, dw_started || jj > 0);
-						}
-					} else {
-						const uint32_t g_tile = s_h0;
-						for (uint32_t jj = 0; jj < WIDTH / 16; ++jj) umma_f16_ss(tmem_acc, kmaj(g_tile, jj), mnmaj(s_w0, jj), IDESC_DGRAD, jj > 0);
-						const uint32_t dw = tmem_base + 64u;
-						for (uint32_t jj = 0; jj < TILE_M / 16; ++jj) umma_f16_ss(dw, mnmaj(g_tile, jj), mnmaj(enc_cur, jj), IDESC_WGRAD, dw_started || jj > 0);
-						umma_commit(bar_enc_free + 8 * e);  // last reader of this enc buffer: release it to the memory group
+				// ---- MMAs of batch b (the weight gradients first: the epilogue below overwrites h_{l-1} with g_{l-1} in place)
+				if (b < NH) {
+					mma64(b == 0 ? enc_cur : s_h0 + (b - 1) * TILE_BYTES, s_w0 + b * (WIDTH * 128), b == 0 ? in_w / 16 : WIDTH / 16, false);
+					if (!TRAIN && b == 0) warp_arrive(bar_enc_free + 8 * e);  // inference: L0 is the only reader of enc
+				} else if (b == NH) {
+					wgmma_fence();
+#pragma unroll
+					for (uint32_t mh = 0; mh < 2; ++mh) {
+						float(&a16)[8] = reinterpret_cast<float(&)[8]>(acc[mh][0]);
+						for (uint32_t jj = 0; jj < WIDTH / 16; ++jj) Wgmma<16>::ss<0, 0>(a16, kmaj(s_h0 + (NH - 1) * TILE_BYTES + mh * 8192u, jj), kmaj(s_wout, jj), jj > 0);
 					}
-					umma_commit(bar_mma);
-					if (b == 1 || b == NH + 1) WS_STAMP(0, k, b == 1 ? 8 : 13);
+					wgmma_commit();
+					wgmma_wait<0>();
+					reg_fence(reinterpret_cast<float(&)[8]>(acc[0][0]));
+					reg_fence(reinterpret_cast<float(&)[8]>(acc[1][0]));
+				} else if (b <= 2 * NH) {
+					const uint32_t l = 2 * NH + 1 - b;
+					const uint32_t h_prev = s_h0 + (l - 1) * TILE_BYTES;
+					if (l == NH) {
+						wgrad(NH, h_prev, s_dy);
+						mma64(s_dy, s_wout, 1, true);
+					} else {
+						const uint32_t g_tile = s_h0 + l * TILE_BYTES;
+						wgrad(l, g_tile, h_prev);
+						mma64(g_tile, s_w0 + l * (WIDTH * 128), WIDTH / 16, true);
+					}
+				} else {
+					wgrad(0, s_h0, enc_cur);
+					mma64(s_h0, s_w0, WIDTH / 16, true);
+					warp_arrive(bar_enc_free + 8 * e);  // last reader of this enc buffer: release it to the memory group
 				}
-				__syncwarp();
-				wait_mma();
+				// From the output layer on, the epilogue writes a tile that this batch's products have read: the staging tile of the
+				// inference output (h_{NH-1}), h_{l-1} (dgrad overwrites it with g_{l-1} after the wgrad read it), the parked
+				// dL/d(enc) rows in the enc tile (read by the dW_0 product). wgmma.wait_group covers only the calling warp's share of
+				// a product, and every warp's share reads all 128 rows of an MN-major operand: the four warps meet here first.
+				if (b >= NH) named_bar_sync(1, WS_MLP_THREADS);
 				if (tid == 0 && (b == 1 || b == NH + 1)) WS_STAMP(0, k, b == 1 ? 9 : 14);
 
-				// ---- epilogue of batch b: this thread owns row `row`, all 64 accumulator columns (two passes of 32)
+				// ---- epilogue of batch b on the accumulator fragment
 				if (b < NH) {
 					const uint32_t h_tile = s_h0 + b * TILE_BYTES;
-					// both halves of the accumulator row are requested before the single wait (one TMEM round trip, not two)
-					uint32_t racc[2][32];
-					tmem_ld_32x32b_x32(tmem_acc + lane_field, racc[0]);
-					tmem_ld_32x32b_x32(tmem_acc + lane_field + 32, racc[1]);
-					tmem_ld_wait();
 #pragma unroll
-					for (uint32_t half = 0; half < 2; ++half) {
-						const uint32_t(&r)[32] = racc[half];
+					for (uint32_t mh = 0; mh < 2; ++mh) {
 #pragma unroll
-						for (uint32_t c = 0; c < 4; ++c) {
-							const uint32_t v0 = act_pack(hid_act, r[c * 8 + 0], r[c * 8 + 1]), v1 = act_pack(hid_act, r[c * 8 + 2], r[c * 8 + 3]);
-							const uint32_t v2 = act_pack(hid_act, r[c * 8 + 4], r[c * 8 + 5]), v3 = act_pack(hid_act, r[c * 8 + 6], r[c * 8 + 7]);
-							st_shared_v4(h_tile + sw128(row, half * 4 + c), v0, v1, v2, v3);
-							if (p.dbg_hidden) *reinterpret_cast<uint4*>(p.dbg_hidden + ((size_t)b * p.batch_size + osample) * 64 + (half * 4 + c) * 8) = make_uint4(v0, v1, v2, v3);
+						for (uint32_t hi = 0; hi < 2; ++hi) {
+							const uint32_t r = frow(mh, hi);
+#pragma unroll
+							for (uint32_t i = 0; i < 8; ++i) {
+								const uint32_t v = act_pack(hid_act, __float_as_uint(acc[mh][4 * i + 2 * hi]), __float_as_uint(acc[mh][4 * i + 2 * hi + 1]));
+								asm volatile("st.shared.b32 [%0], %1;" ::"r"(h_tile + sw128(r, i) + 4u * ft), "r"(v) : "memory");
+								if (p.dbg_hidden) *reinterpret_cast<uint32_t*>(p.dbg_hidden + ((size_t)b * p.batch_size + sample_of(tile, r)) * 64 + 8 * i + 2 * ft) = v;
+							}
 						}
 					}
 				} else if (b == NH) {
-					uint32_t r[16];
-					tmem_ld_32x32b_x16(tmem_acc + lane_field, r);
-					tmem_ld_wait();
-					__half y16[16];
+					// the fp16-rounded outputs go through the row-major staging tile (dy in training, the last hidden layer's tile --
+					// which the output MMA has finished reading -- in inference) to the thread that owns the row
+					const uint32_t stg = TRAIN ? s_dy : s_h0 + (NH - 1) * TILE_BYTES;
 #pragma unroll
-					for (uint32_t q = 0; q < 16; ++q) y16[q] = act_fwd_h(out_act, __float2half_rn(__uint_as_float(r[q])));
+					for (uint32_t mh = 0; mh < 2; ++mh) {
+#pragma unroll
+						for (uint32_t hi = 0; hi < 2; ++hi) {
+#pragma unroll
+							for (uint32_t i = 0; i < 2; ++i) {
+								const uint32_t v = pack_half2(acc[mh][4 * i + 2 * hi], acc[mh][4 * i + 2 * hi + 1]);
+								asm volatile("st.shared.b32 [%0], %1;" ::"r"(stg + sw128(frow(mh, hi), i) + 4u * ft), "r"(v) : "memory");
+							}
+						}
+					}
+					named_bar_sync(1, WS_MLP_THREADS);
+					__half y16[16];
+					{
+						uint4 lo, hi;
+						ld_shared_v4(stg + sw128(row, 0), lo.x, lo.y, lo.z, lo.w);
+						ld_shared_v4(stg + sw128(row, 1), hi.x, hi.y, hi.z, hi.w);
+						*reinterpret_cast<uint4*>(&y16[0]) = lo;
+						*reinterpret_cast<uint4*>(&y16[8]) = hi;
+					}
+#pragma unroll
+					for (uint32_t q = 0; q < 16; ++q) y16[q] = act_fwd_h(out_act, y16[q]);
 					if (p.out_fp16) {
 						uint4* dst = reinterpret_cast<uint4*>(p.out_fp16 + (size_t)osample * 16);
 						dst[0] = *reinterpret_cast<uint4*>(&y16[0]);
@@ -543,24 +616,23 @@ __global__ void __launch_bounds__(WS_THREADS, 1) fused_ws_kernel(const FusedStep
 						}
 					}
 				} else if (b <= 2 * NH) {
-					// g overwrites h in place: each thread rewrites the chunk of its own row it has just read
+					// g overwrites h in place: each thread rewrites the words of the fragment it has just read
 					const uint32_t l = 2 * NH + 1 - b;
 					const uint32_t h_tile = s_h0 + (l - 1) * TILE_BYTES;
-					uint32_t racc[2][32];
-					tmem_ld_32x32b_x32(tmem_acc + lane_field, racc[0]);
-					tmem_ld_32x32b_x32(tmem_acc + lane_field + 32, racc[1]);
-					tmem_ld_wait();
 #pragma unroll
-					for (uint32_t half = 0; half < 2; ++half) {
-						const uint32_t(&r)[32] = racc[half];
+					for (uint32_t mh = 0; mh < 2; ++mh) {
 #pragma unroll
-						for (uint32_t c = 0; c < 4; ++c) {
-							uint32_t f0, f1, f2, f3;
-							ld_shared_v4(h_tile + sw128(row, half * 4 + c), f0, f1, f2, f3);
-							const uint32_t v0 = act_bwd_pack(hid_act, r[c * 8 + 0], r[c * 8 + 1], f0), v1 = act_bwd_pack(hid_act, r[c * 8 + 2], r[c * 8 + 3], f1);
-							const uint32_t v2 = act_bwd_pack(hid_act, r[c * 8 + 4], r[c * 8 + 5], f2), v3 = act_bwd_pack(hid_act, r[c * 8 + 6], r[c * 8 + 7], f3);
-							st_shared_v4(h_tile + sw128(row, half * 4 + c), v0, v1, v2, v3);
-							if (p.dbg_grad_hidden) *reinterpret_cast<uint4*>(p.dbg_grad_hidden + ((size_t)(l - 1) * p.batch_size + osample) * 64 + (half * 4 + c) * 8) = make_uint4(v0, v1, v2, v3);
+						for (uint32_t hi = 0; hi < 2; ++hi) {
+							const uint32_t r = frow(mh, hi);
+#pragma unroll
+							for (uint32_t i = 0; i < 8; ++i) {
+								const uint32_t addr = h_tile + sw128(r, i) + 4u * ft;
+								uint32_t f;
+								asm volatile("ld.shared.b32 %0, [%1];" : "=r"(f) : "r"(addr) : "memory");
+								const uint32_t v = act_bwd_pack(hid_act, __float_as_uint(acc[mh][4 * i + 2 * hi]), __float_as_uint(acc[mh][4 * i + 2 * hi + 1]), f);
+								asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+								if (p.dbg_grad_hidden) *reinterpret_cast<uint32_t*>(p.dbg_grad_hidden + ((size_t)(l - 1) * p.batch_size + sample_of(tile, r)) * 64 + 8 * i + 2 * ft) = v;
+							}
 						}
 					}
 				} else {
@@ -569,66 +641,36 @@ __global__ void __launch_bounds__(WS_THREADS, 1) fused_ws_kernel(const FusedStep
 					if (tid == 0) WS_STAMP(0, k, 3);
 					if (j >= 1) mbar_wait(bar_park_free + 8 * g, (j - 1) & 1u);  // scatter of tile k-2 has consumed park[g]
 					if (tid == 0) WS_STAMP(0, k, 4);
-					uint32_t racc[2][32];
-					tmem_ld_32x32b_x32(tmem_acc + lane_field, racc[0]);
-					tmem_ld_32x32b_x32(tmem_acc + lane_field + 32, racc[1]);
-					tmem_ld_wait();
 #pragma unroll
-					for (uint32_t half = 0; half < 2; ++half) {
-						const uint32_t(&r)[32] = racc[half];
+					for (uint32_t mh = 0; mh < 2; ++mh) {
 #pragma unroll
-						for (uint32_t c = 0; c < 4; ++c) {
-							const uint32_t v0 = pack_half2(__uint_as_float(r[c * 8 + 0]), __uint_as_float(r[c * 8 + 1]));
-							const uint32_t v1 = pack_half2(__uint_as_float(r[c * 8 + 2]), __uint_as_float(r[c * 8 + 3]));
-							const uint32_t v2 = pack_half2(__uint_as_float(r[c * 8 + 4]), __uint_as_float(r[c * 8 + 5]));
-							const uint32_t v3 = pack_half2(__uint_as_float(r[c * 8 + 6]), __uint_as_float(r[c * 8 + 7]));
-							if ((half * 4 + c) * 8 < in_w) st_shared_v4(park_addr(g, row, half * 4 + c), v0, v1, v2, v3);
-							if (p.dbg_denc) *reinterpret_cast<uint4*>(p.dbg_denc + (size_t)osample * 64 + (half * 4 + c) * 8) = make_uint4(v0, v1, v2, v3);
+						for (uint32_t hi = 0; hi < 2; ++hi) {
+							const uint32_t r = frow(mh, hi);
+#pragma unroll
+							for (uint32_t i = 0; i < 8; ++i) {
+								const uint32_t v = pack_half2(acc[mh][4 * i + 2 * hi], acc[mh][4 * i + 2 * hi + 1]);
+								if (i * 8 < in_w) asm volatile("st.shared.b32 [%0], %1;" ::"r"(park_addr(g, r, i) + 4u * ft), "r"(v) : "memory");
+								if (p.dbg_denc) *reinterpret_cast<uint32_t*>(p.dbg_denc + (size_t)sample_of(tile, r) * 64 + 8 * i + 2 * ft) = v;
+							}
 						}
 					}
-					__syncwarp();
-					if ((tid & 31u) == 0) mbar_arrive(bar_park_full + 8 * g);
+					warp_arrive(bar_park_full + 8 * g);
 					if (tid == 0) WS_STAMP(0, k, 5);
 				}
 			}
 		}
 
 		pdl_launch_dependents();
-		// ---- flush the weight-gradient accumulators and the loss
+		// ---- flush the weight-gradient sums and the loss
 		if (TRAIN) {
-			tmem_ld_wait();
-			tc_fence_before_sync();
 			named_bar_sync(1, WS_MLP_THREADS);
-			tc_fence_after_sync();
-			if (dw_started) {
-				// M = 64 accumulators: row m lives in TMEM lane (m % 16) + 32 * (m / 16) -> lanes 0..15 of each lane quadrant
-				const uint32_t lane = tid & 31u;
-				const uint32_t m = warp * 16 + lane;
+			if (dw_smem && dw_started) {
 				for (uint32_t l = 0; l <= NH; ++l) {
-					const uint32_t dw = tmem_base + 64u * (1 + l) + lane_field;
-#pragma unroll
-					for (uint32_t half = 0; half < 2; ++half) {
-						uint32_t r[32];
-						tmem_ld_32x32b_x32(dw + half * 32, r);
-						tmem_ld_wait();
-						if (lane < 16 && m < p.width) {
-							if (l == 0) {
-								float* dst = p.dw_accum + m * in_w;
-#pragma unroll
-								for (uint32_t q = 0; q < 32; q += 4) {
-									const uint32_t n = half * 32 + q;
-									if (n < in_w) red_add_v4_f32(dst + n, __uint_as_float(r[q]), __uint_as_float(r[q + 1]), __uint_as_float(r[q + 2]), __uint_as_float(r[q + 3]));
-								}
-							} else if (l < NH) {
-								float* dst = p.dw_accum + p.width * in_w + (l - 1) * p.width * p.width + m * p.width + half * 32;
-#pragma unroll
-								for (uint32_t q = 0; q < 32; q += 4) if (half * 32 + q < p.width) red_add_v4_f32(dst + q, __uint_as_float(r[q]), __uint_as_float(r[q + 1]), __uint_as_float(r[q + 2]), __uint_as_float(r[q + 3]));
-							} else if (half == 0) {
-								float* dst = p.dw_accum + p.width * in_w + (NH - 1) * p.width * p.width;
-#pragma unroll
-								for (uint32_t n = 0; n < 16; ++n) red_add_f32(dst + n * p.width + m, __uint_as_float(r[n]));
-							}
-						}
+					for (uint32_t i = 0; i < (l == NH ? 2u : 8u); ++i) {
+						uint32_t x[4];
+						ld_shared_v4(s_dw + l * WS_DW_BYTES + (i * WS_MLP_THREADS + tid) * 16u, x[0], x[1], x[2], x[3]);
+						const float v[4] = {__uint_as_float(x[0]), __uint_as_float(x[1]), __uint_as_float(x[2]), __uint_as_float(x[3])};
+						flush_dw(l, i, v);
 					}
 				}
 			}
@@ -636,20 +678,12 @@ __global__ void __launch_bounds__(WS_THREADS, 1) fused_ws_kernel(const FusedStep
 			for (uint32_t o = 16; o > 0; o >>= 1) loss_acc += __shfl_xor_sync(0xFFFFFFFFu, loss_acc, o);
 			if ((tid & 31u) == 0 && p.loss_sum) atomicAdd(p.loss_sum, loss_acc);
 		}
-		tmem_ld_wait();
-		tc_fence_before_sync();
 	}
-
-	__syncthreads();
-	if (warp == 0) tmem_dealloc(tmem_base, tmem_cols);
 }
 
 // ------------------------------------------------------------------------------------------------------------------
 size_t fused_ws_smem_bytes(uint32_t n_hidden_layers, uint32_t enc_width, bool train) {
-	const size_t enc_tiles = WS_ENC_BUFFERS;
-	const bool park_in_enc = enc_tiles == 2 && enc_width <= 32;
-	const size_t tiles = enc_tiles + n_hidden_layers + (train ? (park_in_enc ? 1 : 3) : 0);
-	return tiles * TILE_BYTES + n_hidden_layers * (WIDTH * 128) + 16 * 128 + 128 /* barriers, TMEM slot */;
+	return fused_ws_base_smem_bytes(n_hidden_layers, enc_width, train) + (train && fused_ws_dw_in_smem(n_hidden_layers, enc_width) ? fused_ws_dw_bytes(n_hidden_layers) : 0);
 }
 
 template <uint32_t D, bool TRAIN, bool GENERIC>

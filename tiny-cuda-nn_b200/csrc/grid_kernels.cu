@@ -10,7 +10,7 @@
 //   dy_dx + kernel_grid_backward_input  grid.h:170-212,322-350  summed over features in feature order, fp32
 // Index arithmetic is shared with the fused kernel (grid_device.cuh) and bit-exact with the reference.
 // HBM/L2-bound scattered 2..16-byte accesses. Thread <-> (sample, level) with the level fastest (the reference runs one block row per
-// level to keep a level's table hot in a small L2, grid.h:769-771; the whole table fits B200's L2, and level-fastest makes the
+// level to keep a level's table hot in a small L2, grid.h:769-771; the whole table of the benchmarked configuration nearly fits the H100's 50 MB L2, and level-fastest makes the
 // feature-row accesses whole sectors).
 #include "grid_kernels.h"
 

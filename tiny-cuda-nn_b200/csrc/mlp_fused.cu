@@ -1,4 +1,4 @@
-// mlp_fused.cu -- stand-alone FullyFusedMLP forward / inference on tcgen05: the tensor-core-bound kernel of the hot path.
+// mlp_fused.cu -- stand-alone FullyFusedMLP forward / inference on wgmma: the tensor-core-bound kernel of the general path.
 //
 // Replaces the reference's kernel_mlp_fused<WIDTH, ..., INFERENCE> (fully_fused_mlp.cu:499-557: threadblock_input_layer_forward_dynamic
 // :315-419, threadblock_layer :47-129, threadblock_last_layer_forward :421-476) for Network<T>::inference_mixed_precision
@@ -9,22 +9,16 @@
 // layer of every block (HMMA.F16). Here, per persistent CTA (one per SM):
 //
 //   * weights are loaded ONCE with TMA (cp.async.bulk.tensor, SWIZZLE_128B boxes of 64 K-elements) into shared memory and stay
-//     there as the K-major B operands of every tile; networks with more matrices than fit (128 wide: > 7) stream them through
+//     there as the K-major B operands of every tile; networks with more matrices than fit (128 wide: > 6) stream them through
 //     the same stages as a ring (w_full / w_free mbarriers);
-//   * activations NEVER touch shared memory: layer l accumulates D = A_l . W_l^T in tensor memory (fp32), the epilogue warps read
-//     the accumulator row with tcgen05.ld, apply the activation in fp16 (as warp_activation<__half>, common_device.h:110-215),
-//     and write the packed fp16 row back INTO tensor memory with tcgen05.st, where the next layer's tcgen05.mma reads it as its A
-//     operand (A-from-TMEM). The network input itself enters that way: global -> registers -> tcgen05.st, prefetched a tile ahead;
-//   * SLOTS independent 128-sample tiles are in flight per CTA (2 for 128-wide layers, 4 below; each owns two accumulator regions
-//     that alternate between layers), so that the single MMA-issuing thread always has a tile whose operand is ready while the
-//     epilogue warps of the others convert: the tensor pipe idles only for what the slowest slot's epilogue exceeds the other
-//     slots' MMA time.
+//   * activations NEVER touch shared memory: each consumer warpgroup owns a 64-sample unit of the batch; layer l accumulates
+//     D = A_l . W_l^T in registers (fp32, wgmma m64nNk16), the warpgroup applies the activation in fp16 (as
+//     warp_activation<__half>, common_device.h:110-215) and packs the result straight into the register fragment the next
+//     layer's wgmma reads as its A operand (the accumulator and A fragments of wgmma share the row / column assignment);
+//   * WGS consumer warpgroups work on independent units, so that one warpgroup's epilogue overlaps another's MMAs.
 //
-// Warp roles: warps 4s .. 4s+3 = epilogue / load / store warps of slot s (thread t <-> tile row t <-> TMEM lane t);
-//             warp 4*SLOTS     = MMA issuer (one elected lane) + TMEM allocation;  warp 4*SLOTS + 1 = TMA producer (weights).
-// mbarriers:  a_ready[s][h] (4 arrivals, one per epilogue warp: half h of the A operand of this slot's next layer is in tensor memory)
-//             acc_ready[s] (tcgen05.commit: the accumulator of this slot's current layer is complete)
-//             w_full[stage] (TMA complete_tx), w_free[stage] (SLOTS arrivals by tcgen05.commit: ring mode only)
+// Warp roles: warpgroups 0 .. WGS-1 = consumers (one 64-sample unit at a time); the last warp = TMA producer (weights).
+// mbarriers:  w_full[stage] (TMA complete_tx), w_free[stage] (one arrival per consumer warp: ring mode only)
 //
 // Numerics: fp16 operands, fp32 accumulation, ONE rounding to fp16 per layer (the reference accumulates in fp16 inside HMMA;
 // tolerance statement in DESIGN.md section 4).
@@ -43,79 +37,39 @@ using namespace fused;
 namespace {
 
 constexpr uint32_t MLPF_MAX_STAGES = 32;
+constexpr uint32_t UNIT_M = 64;  // samples per consumer warpgroup and MMA
 
 template <uint32_t W>
 struct MlpCfg {
-	static constexpr uint32_t SLOTS = W == 128 ? 2 : 4;        // 128-sample tiles in flight per CTA
-	static constexpr uint32_t GROUPS = W == 128 ? 2 : 1;       // epilogue warp groups (4 warps) per slot: each owns W / GROUPS columns of every row
-	static constexpr uint32_t SLOT_WARPS = 4 * GROUPS;
-	static constexpr uint32_t EPI_WARPS = SLOTS * SLOT_WARPS;  // 16
-	static constexpr uint32_t THREADS = (EPI_WARPS + 2) * 32;  // 576
-	static constexpr uint32_t REGION = W < 32 ? 32 : W;        // TMEM columns of one accumulator region
-	static constexpr uint32_t TMEM_COLS = SLOTS * 2 * REGION;  // 512 / 512 / 256 / 256
+	static constexpr uint32_t WGS = W == 128 ? 2 : 4;          // consumer warpgroups
+	static constexpr uint32_t THREADS = WGS * 128 + 32;        // + the TMA producer warp
+	static constexpr uint32_t ACC_N = W < 32 ? 32 : W;         // accumulator columns: the widest product of the chain (dL/d(input) of
+	                                                           // a 16-wide network is up to 32 wide)
+	static constexpr uint32_t KMAX = W == 128 ? 128 : 64;      // widest K (the network input may be wider than the layers)
 	static constexpr uint32_t KBLOCKS = (W + 63) / 64;         // 64-element K blocks of a weight stage
 	static constexpr uint32_t KBLOCK_BYTES = W * 128;          // [W rows][64 fp16], SWIZZLE_128B
 	static constexpr uint32_t STAGE_BYTES = KBLOCKS * KBLOCK_BYTES < 2048 ? 2048 : KBLOCKS * KBLOCK_BYTES;
-	static constexpr uint32_t GROUP_COLS = W / GROUPS;         // accumulator columns a thread converts per hidden layer (<= 64)
-	static constexpr uint32_t PIECE = GROUP_COLS < 32 ? GROUP_COLS : 32;  // ... in pieces of one tcgen05.ld
-	static constexpr uint32_t N_PIECES = GROUP_COLS / PIECE;
 };
 
 struct MlpKernelParams {
 	MlpForwardParams p;
 	uint32_t n_stages;  // == n_steps when all matrices are resident
 	uint32_t resident;
-	uint32_t n_steps;   // MMAs chained per tile: n_hidden_layers + 1 (the backward chain without dL/d(input): n_hidden_layers)
+	uint32_t n_steps;   // MMAs chained per unit: n_hidden_layers + 1 (the backward chain without dL/d(input): n_hidden_layers)
 };
-
-template <uint32_t N>
-__device__ __forceinline__ void tmem_ld_n(uint32_t taddr, uint32_t (&r)[N]);
-template <>
-__device__ __forceinline__ void tmem_ld_n<16>(uint32_t taddr, uint32_t (&r)[16]) { tmem_ld_32x32b_x16(taddr, r); }
-template <>
-__device__ __forceinline__ void tmem_ld_n<32>(uint32_t taddr, uint32_t (&r)[32]) { tmem_ld_32x32b_x32(taddr, r); }
-template <uint32_t N>
-__device__ __forceinline__ void tmem_st_n(uint32_t taddr, const uint32_t (&r)[N]);
-template <>
-__device__ __forceinline__ void tmem_st_n<8>(uint32_t taddr, const uint32_t (&r)[8]) { tmem_st_32x32b_x8(taddr, r); }
-template <>
-__device__ __forceinline__ void tmem_st_n<16>(uint32_t taddr, const uint32_t (&r)[16]) { tmem_st_32x32b_x16(taddr, r); }
-
-// 8 x 8 transpose of 128-bit elements across every aligned group of 8 lanes (butterfly over lane bits 2, 1, 0): on return a[j] of
-// lane l8 holds what a[l8] of lane j held. The network input and output are rows of up to 256 bytes per sample and a thread owns a
-// whole row (it owns the matching TMEM lane); moving rows between global memory and a thread one 16-byte piece per lane would make
-// every warp-level access touch 32 different cache lines (measured: the uncoalesced version spent more time in the LSU than in the
-// tensor pipe). Instead 8 lanes fetch 8 consecutive 16-byte pieces of ONE row -- 128 contiguous bytes -- for 8 rows in turn, and this
-// transpose hands every lane the pieces of its own row (and the reverse for the output).
-__device__ __forceinline__ void transpose8x8_u128(uint4 (&a)[8], uint32_t lane) {
-#pragma unroll
-	for (uint32_t s = 4; s >= 1; s >>= 1) {
-		const bool upper = (lane & s) != 0;
-#pragma unroll
-		for (uint32_t j = 0; j < 8; ++j) {
-			if (j & s) continue;  // pair (j, j | s): lower lanes keep a[j] and trade a[j | s], upper lanes the other way round
-			const uint4 send = upper ? a[j] : a[j | s];
-			uint4 recv;
-			recv.x = __shfl_xor_sync(0xFFFFFFFFu, send.x, s);
-			recv.y = __shfl_xor_sync(0xFFFFFFFFu, send.y, s);
-			recv.z = __shfl_xor_sync(0xFFFFFFFFu, send.z, s);
-			recv.w = __shfl_xor_sync(0xFFFFFFFFu, send.w, s);
-			if (upper) a[j] = recv;
-			else a[j | s] = recv;
-		}
-	}
-}
 
 }  // namespace
 
-// Phase stamps for scripts/mlp_timeline.py: [cta][role: 0 = MMA issuer, 1 + s = epilogue warp 0 of slot s][event 0..63][field 0..7].
+// Phase stamps (tcnnb_network_debug_clocks, profiling only): [cta][role = consumer warpgroup 0..3, 4 unused][event = round * n_steps +
+// step, < 64][field: 0 = waiting for the weights, 1 = weights ready, 2 = product complete, 3 = epilogue done], written by the first
+// thread of the warpgroup.
 #define MLPF_STAMP(role, event, field)                                                                                               \
 	do {                                                                                                                             \
 		if (p.dbg_clock && (event) < 64u) p.dbg_clock[(((size_t)blockIdx.x * 5u + (role)) * 64u + (event)) * 8u + (field)] = clock64(); \
 	} while (0)
 
-// 576 threads per CTA -> 96 registers per thread (what the register file's allocation granularity leaves; asking for 112 with
-// __maxnreg__ compiles but does not launch). The accumulator pieces of the widest kernels spill a few words to local memory.
+// The chain of one 64-sample unit in one consumer warpgroup. Thread (warp w of the group, lane) owns rows r0 = 16 w + lane / 4 and
+// r0 + 8 of the unit, and the column pairs 8 i + 2 (lane % 4) of every accumulator / A fragment (ptx.cuh, Wgmma).
 //
 // BWD = true is the same machine run backwards (threadblock_layer<..., BACKWARD>, fully_fused_mlp.cu:47-129,151-259): the operand that
 // enters is dL/d(output) (already through the output activation's transfer), step j multiplies by matrix NH - j read MN-major
@@ -144,46 +98,30 @@ mlp_forward_kernel(const MlpKernelParams kp, const __grid_constant__ CUtensorMap
 	if (smem_base & 1023u) __trap();
 	const uint32_t s_stage0 = smem_base;
 	const uint32_t s_bars = s_stage0 + n_stages * C::STAGE_BYTES;
-	const uint32_t bar_w_full = s_bars;                               // [MLPF_MAX_STAGES]
-	const uint32_t bar_w_free = bar_w_full + 8 * MLPF_MAX_STAGES;     // [MLPF_MAX_STAGES]
-	const uint32_t bar_a_ready = bar_w_free + 8 * MLPF_MAX_STAGES;    // [4]
-	const uint32_t bar_acc_ready = bar_a_ready + 8 * 4;               // [4]
-	const uint32_t s_tmem_slot = bar_acc_ready + 8 * 4;
+	const uint32_t bar_w_full = s_bars;                            // [MLPF_MAX_STAGES]
+	const uint32_t bar_w_free = bar_w_full + 8 * MLPF_MAX_STAGES;  // [MLPF_MAX_STAGES]
 
 	if (tid == 0) {
 		for (uint32_t i = 0; i < n_stages; ++i) {
 			mbar_init(bar_w_full + 8 * i, 1);
-			mbar_init(bar_w_free + 8 * i, C::SLOTS);
-		}
-		for (uint32_t s = 0; s < C::SLOTS; ++s) {
-			mbar_init(bar_a_ready + 8 * s, C::SLOT_WARPS);
-			mbar_init(bar_acc_ready + 8 * s, 1);
+			mbar_init(bar_w_free + 8 * i, C::WGS * 4);
 		}
 		fence_mbar_init();
 	}
-	if (warp == C::EPI_WARPS) {
-		__syncwarp();
-		tmem_alloc(s_tmem_slot, C::TMEM_COLS);
-		tmem_relinquish();
-	}
-	if (warp == C::EPI_WARPS + 1 && lane == 0) {
+	if (warp == C::WGS * 4 && lane == 0) {
 		tma_prefetch_desc(&map_w0);
 		tma_prefetch_desc(&map_wh);
 		tma_prefetch_desc(&map_wo);
 	}
-	tc_fence_before_sync();
 	__syncthreads();
-	tc_fence_after_sync();
 	pdl_wait();  // from here on global memory written by the previous kernel on the stream is read
 
-	uint32_t tmem_base;
-	asm volatile("ld.shared.b32 %0, [%1];" : "=r"(tmem_base) : "r"(s_tmem_slot));
-	const uint32_t n_tiles = p.batch_size / TILE_M;
-	// tiles of this CTA: blockIdx.x + j * gridDim.x, j = 0 .. n_my - 1; slot s owns j = s, s + SLOTS, ...
-	const uint32_t n_my = blockIdx.x < n_tiles ? (n_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
-	const uint32_t n_rounds = (n_my + C::SLOTS - 1) / C::SLOTS;
+	const uint32_t n_units = p.batch_size / UNIT_M;
+	// units of this CTA: blockIdx.x + j * gridDim.x, j = 0 .. n_my - 1; round r gives unit j = r * WGS + s to consumer warpgroup s
+	const uint32_t n_my = blockIdx.x < n_units ? (n_units - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
+	const uint32_t n_rounds = (n_my + C::WGS - 1) / C::WGS;
 
-	if (warp == C::EPI_WARPS + 1) {
+	if (warp == C::WGS * 4) {
 		// =============================================================================== TMA producer: weight matrices -> stages
 		if (lane == 0) {
 			const uint32_t n_loads = resident ? n_layers : n_rounds * n_layers;
@@ -207,332 +145,128 @@ mlp_forward_kernel(const MlpKernelParams kp, const __grid_constant__ CUtensorMap
 				}
 			}
 		}
-	} else if (warp == C::EPI_WARPS) {
-		// =============================================================================== MMA issuer
-		// Per slot: which layer comes next. A slot whose tiles have run out keeps walking the layers of the remaining rounds as a
-		// "virtual" consumer in ring mode: it only releases the weight stages (w_free expects SLOTS arrivals per use).
-		uint32_t layer[C::SLOTS], round[C::SLOTS], a_par[C::SLOTS], n_real[C::SLOTS];
-		uint32_t remaining = 0;
-#pragma unroll
-		for (uint32_t s = 0; s < C::SLOTS; ++s) {
-			layer[s] = round[s] = a_par[s] = 0;
-			n_real[s] = n_my > s ? (n_my - s + C::SLOTS - 1) / C::SLOTS : 0;
-			remaining += (resident ? n_real[s] : n_rounds) * n_layers;
-		}
-		while (remaining) {
-#pragma unroll
-			for (uint32_t s = 0; s < C::SLOTS; ++s) {
-				const uint32_t n_rounds_s = resident ? n_real[s] : n_rounds;
-				if (round[s] >= n_rounds_s) continue;
-				const bool real = round[s] < n_real[s];
-				const uint32_t l = layer[s];
-				const uint32_t g = round[s] * n_layers + l;
-				const uint32_t stage = resident ? l : g % n_stages;
-				const uint32_t w_par = resident ? 0u : (g / n_stages) & 1u;
-				// warp-uniform decisions (every lane tests; the vote makes the result one value)
-				if (real && !__all_sync(0xFFFFFFFFu, mbar_test(bar_a_ready + 8 * s, a_par[s]))) continue;
-				if (!__all_sync(0xFFFFFFFFu, mbar_test(bar_w_full + 8 * stage, w_par))) continue;
-				if (real) {
-					const uint32_t ev = round[s] * n_layers + l;
-					if (lane == 0) MLPF_STAMP(0, ev * C::SLOTS + s, 0);
-					tc_fence_after_sync();
-					if (elect_one_sync()) {
-						const uint32_t slot_base = tmem_base + s * 2 * C::REGION;
-						const uint32_t d_tmem = slot_base + (l & 1u) * C::REGION;
-						const uint32_t a_tmem = slot_base + ((l + 1u) & 1u) * C::REGION;  // first half of the other region
-						const uint32_t b_smem = s_stage0 + stage * C::STAGE_BYTES;
-						const uint32_t ksteps = (l == 0 ? first_w : W) / 16;
-						const uint32_t n_cols = l == NH ? last_w : W;
-						const uint32_t idesc = umma_idesc_f16(128, n_cols, 0, BWD ? 1 : 0);
-						for (uint32_t j = 0; j < ksteps; ++j) {
-							// forward: stage = [N rows][64 K] boxes, K-major; backward: the same boxes are [K rows][64 N], MN-major
-							// (16 K-rows = 2 048 bytes per step, the next 64 N-columns one box further)
-							const uint64_t b_desc = BWD ? umma_desc_sw128(b_smem + j * 2048u, C::KBLOCK_BYTES, 1024u)
-							                            : umma_desc_sw128(b_smem + (j >> 2) * C::KBLOCK_BYTES + (j & 3u) * 32u, 16u, 1024u);
-							umma_f16_ts(d_tmem, a_tmem + j * 8u, b_desc, idesc, j > 0);
-						}
-						umma_commit(bar_acc_ready + 8 * s);
-						if (!resident) umma_commit(bar_w_free + 8 * stage);
-					}
-					__syncwarp();
-					if (lane == 0) MLPF_STAMP(0, ev * C::SLOTS + s, 1);
-					a_par[s] ^= 1u;
-				} else if (lane == 0) {
-					mbar_arrive_plain(bar_w_free + 8 * stage);
-				}
-				if (++layer[s] == n_layers) {
-					layer[s] = 0;
-					++round[s];
-				}
-				--remaining;
-			}
-		}
 	} else {
-		// =============================================================================== epilogue / load / store warps of one slot
-		// SLOT_WARPS warps per slot: warp (grp, wq) owns TMEM lanes 32 wq .. 32 wq + 31 (thread <-> tile row) and the columns
-		// [grp * GROUP_COLS, (grp + 1) * GROUP_COLS) of every accumulator / input / output row of the tile.
-		const uint32_t s = warp / C::SLOT_WARPS, grp = (warp / 4) % C::GROUPS, wq = warp & 3u;
-		const uint32_t row = wq * 32 + lane;
-		const uint32_t lane_field = (wq * 32u) << 16;
-		const uint32_t slot_base = tmem_base + s * 2 * C::REGION + lane_field;
-		const uint32_t col0 = grp * C::GROUP_COLS;  // first accumulator column of this thread
-		const uint32_t g8 = lane >> 3, l8 = lane & 7u;
-		const bool stamp = grp == 0 && wq == 0 && lane == 0;
-		uint32_t acc_par = 0;
-
-		// ---- network input: one 64-column block per warp group. The 8 lanes of a lane group fetch 8 consecutive 16-byte pieces of
-		// ONE row (128 contiguous bytes) for 8 rows in turn; transpose8x8_u128 hands every lane its own row when the tile starts
-		// (one tile later, so that the loads stay in flight across the last layer).
-		const bool has_in_block = col0 < first_w;
-		uint4 pre[8];
-		auto load_input = [&](uint32_t tile) {
-			if (!has_in_block) return;
-			const size_t tile_row0 = (size_t)tile * TILE_M + wq * 32;
-			if (p.input_fp16) {
-				const uint32_t col = col0 + l8 * 8;
+		// =============================================================================== consumer warpgroup s
+		const uint32_t s = warp / 4, wq = warp & 3u;
+		const uint32_t fq = lane >> 2, ft = lane & 3u;
+		const uint32_t r0 = wq * 16 + fq;  // rows r0 and r0 + 8 of the unit
+		const bool stamp = wq == 0 && lane == 0;
+		// In ring mode every consumer walks every round, also past its last unit: it then only releases the weight stages.
+		const uint32_t my_rounds = resident ? (n_my > s ? (n_my - s + C::WGS - 1) / C::WGS : 0) : n_rounds;
+		uint32_t a[C::KMAX / 16][4];      // A fragment of the next product: k-step kk, registers as in Wgmma::rs
+		float acc[C::ACC_N / 2];
+		for (uint32_t r = 0; r < my_rounds; ++r) {
+			const uint32_t j = r * C::WGS + s;
+			const bool real = j < n_my;
+			const size_t row0 = (size_t)(blockIdx.x + j * gridDim.x) * UNIT_M;
+			if (real) {
+				// ---- the rows that enter the chain -> A fragment
 #pragma unroll
-				for (uint32_t jj = 0; jj < 8; ++jj) {
-					pre[jj] = col < first_w ? __ldg(reinterpret_cast<const uint4*>(p.input_fp16 + (tile_row0 + g8 * 8 + jj) * first_w + col)) : make_uint4(0, 0, 0, 0);
-				}
-			} else {
-				// Identity encoding (identity.h:46-67): the first n_input_dims features are the inputs, the padding features are ONE.
-				// A handful of floats per sample: fetched by the owning thread directly, already in row order (no transpose below).
-				const float* src = p.input_fp32 + (tile_row0 + lane) * p.n_input_dims;
+				for (uint32_t kk = 0; kk < C::KMAX / 16; ++kk) {
 #pragma unroll
-				for (uint32_t jj = 0; jj < 8; ++jj) {
-					uint32_t w4[4];
-#pragma unroll
-					for (uint32_t i = 0; i < 4; ++i) {
-						const uint32_t c = col0 + jj * 8 + i * 2;
-						if (c < in_w) {
-							const float lo = c < p.n_input_dims ? __ldg(src + c) : 1.0f;
-							const float hi = c + 1 < p.n_input_dims ? __ldg(src + c + 1) : 1.0f;
-							w4[i] = pack_half2(lo, hi);
-						} else {
-							w4[i] = 0;
-						}
-					}
-					pre[jj] = make_uint4(w4[0], w4[1], w4[2], w4[3]);
-				}
-			}
-		};
-
-		uint32_t j = s;
-		if (j < n_my) load_input(blockIdx.x + j * gridDim.x);
-		for (; j < n_my; j += C::SLOTS) {
-			const uint32_t tile = blockIdx.x + j * gridDim.x;
-			const size_t sample = (size_t)tile * TILE_M + row;
-			const size_t tile_row0 = (size_t)tile * TILE_M + wq * 32;
-			// ---- input row -> tensor memory: A operand of layer 0 lives in the first half of region 1
-			if (has_in_block) {
-				const uint32_t a0 = slot_base + C::REGION + col0 / 2;
-				if (p.input_fp16) transpose8x8_u128(pre, lane);
-#pragma unroll
-				for (uint32_t q = 0; q < 4; ++q) {  // 16 columns of fp16 = 8 TMEM columns per store
-					if (col0 + q * 16 < first_w) {
-						const uint32_t v[8] = {pre[2 * q].x, pre[2 * q].y, pre[2 * q].z, pre[2 * q].w, pre[2 * q + 1].x, pre[2 * q + 1].y, pre[2 * q + 1].z, pre[2 * q + 1].w};
-						tmem_st_n<8>(a0 + q * 8, v);
-					}
-				}
-				tmem_st_wait();
-			}
-			tc_fence_before_sync();
-			__syncwarp();
-			if (lane == 0) mbar_arrive_plain(bar_a_ready + 8 * s);
-
-			for (uint32_t l = 0; l < n_layers; ++l) {
-				// the next tile's input travels while the last layer computes
-				if (l == n_layers - 1 && j + C::SLOTS < n_my) {
-					load_input(blockIdx.x + (j + C::SLOTS) * gridDim.x);
-					if (BWD && l8 == 0) {  // ... and the forward activations its first step will multiply with
-						const size_t next_row0 = (size_t)(blockIdx.x + (j + C::SLOTS) * gridDim.x) * TILE_M + wq * 32;
-						const __half* nxt = p.hidden_in + ((size_t)(NH - 1) * p.batch_size + next_row0 + g8 * 8) * W + col0;
-#pragma unroll
-						for (uint32_t jj = 0; jj < 8; ++jj) asm volatile("prefetch.global.L2 [%0];" ::"l"(nxt + (size_t)jj * W));
-					}
-				}
-				// backward: the forward pass's activations of the layer this step lands on (hidden layer NH - 1 - l), fetched BEFORE the
-				// wait so that the load travels while the MMA runs. ReLU only needs the signs: two bits per fp16 pair.
-				constexpr uint32_t FWD_WORDS = BWD ? (GENERIC_ACT ? C::GROUP_COLS / 2 : 2) : 1;
-				uint32_t fwd[FWD_WORDS];
-				if (BWD && l + 1 < NH && l8 == 0) {
-					// The rows the NEXT step needs are pulled into L2 now (no registers to spare for a deeper register prefetch: the kernel sits at
-					// the 96-register cap): by the time they are loaded they cost an L2 hit instead of a DRAM round trip in front of the epilogue.
-					const __half* nxt = p.hidden_in + ((size_t)(NH - 2 - l) * p.batch_size + tile_row0 + g8 * 8) * W + col0;
-#pragma unroll
-					for (uint32_t jj = 0; jj < 8; ++jj) asm volatile("prefetch.global.L2 [%0];" ::"l"(nxt + (size_t)jj * W));
-				}
-				if (BWD && l < NH) {
-					uint4 hv[C::GROUP_COLS / 8];
-					if (C::GROUP_COLS == 64) {
-						// coalesced: 8 lanes fetch the 8 consecutive 16-byte chunks of ONE row, for 8 rows in turn; the transpose hands every
-						// lane the chunks of its own row
-						const __half* src = p.hidden_in + ((size_t)(NH - 1 - l) * p.batch_size + tile_row0 + g8 * 8) * W + col0 + l8 * 8;
-#pragma unroll
-						for (uint32_t jj = 0; jj < 8; ++jj) hv[jj % (C::GROUP_COLS / 8)] = __ldg(reinterpret_cast<const uint4*>(src + (size_t)jj * W));
-						uint4(&hv8)[8] = reinterpret_cast<uint4(&)[8]>(hv);
-						transpose8x8_u128(hv8, lane);
-					} else {
-						const uint4* src = reinterpret_cast<const uint4*>(p.hidden_in + ((size_t)(NH - 1 - l) * p.batch_size + sample) * W + col0);
-#pragma unroll
-						for (uint32_t i = 0; i < C::GROUP_COLS / 8; ++i) hv[i] = __ldg(src + i);
-					}
-					if (!GENERIC_ACT) fwd[0] = fwd[FWD_WORDS - 1] = 0;
-#pragma unroll
-					for (uint32_t i = 0; i < C::GROUP_COLS / 8; ++i) {
-						const uint4 v = hv[i];
-						const uint32_t w4[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-						for (uint32_t c = 0; c < 4; ++c) {
-							if (GENERIC_ACT) {
-								fwd[(4 * i + c) % FWD_WORDS] = w4[c];
+					for (uint32_t q = 0; q < 4; ++q) {
+						const size_t rr = row0 + r0 + (q & 1u) * 8;
+						const uint32_t c = kk * 16 + (q >> 1) * 8 + 2 * ft;
+						uint32_t v = 0;
+						if (c < first_w) {
+							if (p.input_fp16) {
+								v = __ldg(reinterpret_cast<const uint32_t*>(p.input_fp16 + rr * first_w + c));
 							} else {
-								// positive fp16: sign clear and not zero
-								const uint32_t lo_pos = ((w4[c] & 0x8000u) == 0 && (w4[c] & 0x7FFFu) != 0) ? 1u : 0u;
-								const uint32_t hi_pos = ((w4[c] & 0x80000000u) == 0 && (w4[c] & 0x7FFF0000u) != 0) ? 2u : 0u;
-								fwd[((4 * i + c) / 16) % FWD_WORDS] |= (lo_pos | hi_pos) << (2 * ((4 * i + c) % 16));
+								// Identity encoding (identity.h:46-67): the first n_input_dims features are the inputs, the padding features are ONE
+								const float* src = p.input_fp32 + rr * p.n_input_dims;
+								const float lo = c < p.n_input_dims ? __ldg(src + c) : 1.0f;
+								const float hi = c + 1 < p.n_input_dims ? __ldg(src + c + 1) : 1.0f;
+								v = pack_half2(lo, hi);
 							}
 						}
+						a[kk][q] = v;
 					}
 				}
-				// fp32 accumulator pair `idx` of this thread's columns -> packed fp16 pair after the (derivative of the) activation
-				auto convert = [&](uint32_t idx, uint32_t lo_bits, uint32_t hi_bits) -> uint32_t {
-					if (!BWD) return act_pack(hid_act, lo_bits, hi_bits);
-					if (GENERIC_ACT) return act_bwd_pack(hid_act, lo_bits, hi_bits, fwd[idx % FWD_WORDS]);
-					const uint32_t b = (fwd[(idx / 16) % FWD_WORDS] >> (2 * (idx % 16))) & 3u;
-					__half2 g = __floats2half2_rn(__uint_as_float(lo_bits), __uint_as_float(hi_bits));
-					const uint32_t m = ((b & 1u) ? 0x3C00u : 0u) | ((b & 2u) ? 0x3C000000u : 0u);  // (forward > 0) as 1.0 / 0.0, common_device.h:363-368
-					g = __hmul2(g, *reinterpret_cast<const __half2*>(&m));
-					return *reinterpret_cast<const uint32_t*>(&g);
-				};
-				const uint32_t ev = (j / C::SLOTS) * n_layers + l;
-				if (stamp) MLPF_STAMP(1 + s, ev, 0);
-				mbar_wait(bar_acc_ready + 8 * s, acc_par);
-				acc_par ^= 1u;
-				tc_fence_after_sync();
-				if (stamp) MLPF_STAMP(1 + s, ev, 1);
-				const uint32_t acc = slot_base + (l & 1u) * C::REGION;
-				if (l < NH) {
-					// hidden layer: fp32 accumulator row -> activation in fp16 -> packed pairs, IN PLACE into the first half of this
-					// region, which the next layer's MMA reads as its A operand. Columns [c, c + n) are written to [c / 2, (c + n) / 2):
-					// a group's writes land in columns it has read itself or -- with two groups -- in columns the OTHER group reads,
-					// hence: every thread loads all of its columns first, then the slot's groups meet at a named barrier, then store.
-					// Hazard: group 1's stores (A columns 32..63) land in columns that group 0 still has to READ as accumulator columns
-					// 32..63 (its last piece); group 0's own stores only cover columns it has read itself. So group 0 works piece by piece
-					// and signals a named barrier (bar.arrive, non-blocking) once its last piece is in registers; group 1 converts all
-					// its pieces first and stores them after the barrier.
-					// The rows also go to global memory when the caller keeps them (forward activations / backward g_l): 64-column groups
-					// AFTER the hand-over to the MMA issuer and coalesced through the 8 x 8 lane transpose, narrower ones directly.
-					uint4 keep[C::GROUP_COLS == 64 ? 8 : 1];
-					auto store_piece = [&](uint32_t k, const uint32_t (&h)[C::PIECE / 2]) {
-						tmem_st_n<C::PIECE / 2>(acc + (col0 + k * C::PIECE) / 2, h);
-						if (C::GROUP_COLS == 64) {
-							if (p.hidden_out)
-#pragma unroll
-							for (uint32_t i = 0; i < C::PIECE / 8; ++i) keep[(k * (C::PIECE / 8) + i) % (C::GROUP_COLS == 64 ? 8 : 1)] = make_uint4(h[4 * i], h[4 * i + 1], h[4 * i + 2], h[4 * i + 3]);
-						} else if (p.hidden_out) {
-							uint4* dst = reinterpret_cast<uint4*>(p.hidden_out + ((size_t)(BWD ? NH - 1 - l : l) * p.batch_size + sample) * W + col0 + k * C::PIECE);
-#pragma unroll
-							for (uint32_t i = 0; i < C::PIECE / 8; ++i) dst[i] = make_uint4(h[4 * i], h[4 * i + 1], h[4 * i + 2], h[4 * i + 3]);
-						}
-					};
-					if (C::GROUPS == 1 || grp == 0) {
-#pragma unroll
-						for (uint32_t k = 0; k < C::N_PIECES; ++k) {
-							uint32_t r[C::PIECE], h[C::PIECE / 2];
-							tmem_ld_n<C::PIECE>(acc + col0 + k * C::PIECE, r);
-							tmem_ld_wait();
-							if (C::GROUPS > 1 && k == C::N_PIECES - 1) asm volatile("bar.arrive %0, %1;" ::"r"(1u + s), "r"(C::SLOT_WARPS * 32u) : "memory");
-#pragma unroll
-							for (uint32_t i = 0; i < C::PIECE / 2; ++i) h[i] = convert(k * (C::PIECE / 2) + i, r[2 * i], r[2 * i + 1]);
-							store_piece(k, h);
-						}
-						if (stamp) MLPF_STAMP(1 + s, ev, 2);
-					} else {
-						uint32_t h[C::N_PIECES][C::PIECE / 2];
-#pragma unroll
-						for (uint32_t k = 0; k < C::N_PIECES; ++k) {
-							uint32_t r[C::PIECE];
-							tmem_ld_n<C::PIECE>(acc + col0 + k * C::PIECE, r);
-							tmem_ld_wait();
-#pragma unroll
-							for (uint32_t i = 0; i < C::PIECE / 2; ++i) h[k][i] = convert(k * (C::PIECE / 2) + i, r[2 * i], r[2 * i + 1]);
-						}
-						asm volatile("bar.sync %0, %1;" ::"r"(1u + s), "r"(C::SLOT_WARPS * 32u) : "memory");
-#pragma unroll
-						for (uint32_t k = 0; k < C::N_PIECES; ++k) store_piece(k, h[k]);
-					}
-					if (stamp) MLPF_STAMP(1 + s, ev, 3);
-					tmem_st_wait();
-					tc_fence_before_sync();
+			}
+			for (uint32_t l = 0; l < n_layers; ++l) {
+				const uint32_t g = r * n_layers + l;
+				const uint32_t stage = resident ? l : g % n_stages;
+				if (stamp) MLPF_STAMP(s, g, 0);
+				mbar_wait(bar_w_full + 8 * stage, resident ? 0u : (g / n_stages) & 1u);
+				if (stamp) MLPF_STAMP(s, g, 1);
+				if (!real) {
 					__syncwarp();
-					if (lane == 0) mbar_arrive_plain(bar_a_ready + 8 * s);
-					if (stamp) MLPF_STAMP(1 + s, ev, 4);
-					if (C::GROUP_COLS == 64 && p.hidden_out) {
-						uint4(&keep8)[8] = reinterpret_cast<uint4(&)[8]>(keep);
-						transpose8x8_u128(keep8, lane);
-						__half* dst = p.hidden_out + ((size_t)(BWD ? NH - 1 - l : l) * p.batch_size + tile_row0 + g8 * 8) * W + col0 + l8 * 8;
+					if (lane == 0) mbar_arrive_plain(bar_w_free + 8 * stage);
+					continue;
+				}
+				// backward: the forward pass's activations of the layer this step lands on (hidden layer NH - 1 - l), fetched before
+				// the MMA so that the loads travel while it runs
+				uint32_t fwd[BWD ? W / 4 : 1];
+				if (BWD && l < NH) {
+					const __half* hsrc = p.hidden_in + ((size_t)(NH - 1 - l) * p.batch_size + row0 + r0) * W + 2 * ft;
 #pragma unroll
-						for (uint32_t jj = 0; jj < 8; ++jj) *reinterpret_cast<uint4*>(dst + (size_t)jj * W) = keep8[jj];
+					for (uint32_t i = 0; i < W / 8; ++i) {
+						fwd[2 * i] = __ldg(reinterpret_cast<const uint32_t*>(hsrc + 8 * i));
+						fwd[2 * i + 1] = __ldg(reinterpret_cast<const uint32_t*>(hsrc + 8 * W + 8 * i));
+					}
+				}
+				// ---- D = A . B: forward: the stage holds [N rows][64 K] boxes, K-major; backward: the same boxes are [K rows][64 N],
+				// MN-major (16 K-rows = 2 048 bytes per step, the next 64 N-columns one box further)
+				const uint32_t b_smem = s_stage0 + stage * C::STAGE_BYTES;
+				const uint32_t ksteps = (l == 0 ? first_w : W) / 16;
+				// every product is N = W wide except dL/d(input) of a 16-wide network, which may be 32 wide
+				const bool wide = C::ACC_N != W && BWD && l == NH;
+				wgmma_fence();
+#pragma unroll
+				for (uint32_t kk = 0; kk < C::KMAX / 16; ++kk) {
+					if (kk < ksteps) {
+						const uint64_t b_desc = BWD ? wgmma_desc_sw128(b_smem + kk * 2048u, C::KBLOCK_BYTES, 1024u)
+						                            : wgmma_desc_sw128(b_smem + (kk >> 2) * C::KBLOCK_BYTES + (kk & 3u) * 32u, 16u, 1024u);
+						if (wide) Wgmma<C::ACC_N>::template rs<BWD ? 1 : 0>(acc, a[kk], b_desc, kk > 0);
+						else Wgmma<W>::template rs<BWD ? 1 : 0>(reinterpret_cast<float(&)[W / 2]>(acc), a[kk], b_desc, kk > 0);
+					}
+				}
+				wgmma_commit();
+				wgmma_wait<0>();
+				reg_fence(acc);
+				if (stamp) MLPF_STAMP(s, g, 2);
+				if (!resident) {
+					__syncwarp();
+					if (lane == 0) mbar_arrive_plain(bar_w_free + 8 * stage);
+				}
+				if (l < NH) {
+					// hidden layer: fp32 accumulator -> (derivative of the) activation in fp16 -> the next product's A fragment; the rows
+					// also go to global memory when the caller keeps them (forward activations / backward g_l)
+					__half* keep = p.hidden_out ? p.hidden_out + ((size_t)(BWD ? NH - 1 - l : l) * p.batch_size + row0 + r0) * W + 2 * ft : nullptr;
+#pragma unroll
+					for (uint32_t i = 0; i < W / 8; ++i) {
+#pragma unroll
+						for (uint32_t hi = 0; hi < 2; ++hi) {
+							const uint32_t lo_bits = __float_as_uint(acc[4 * i + 2 * hi]), hi_bits = __float_as_uint(acc[4 * i + 2 * hi + 1]);
+							const uint32_t v = BWD ? act_bwd_pack(hid_act, lo_bits, hi_bits, fwd[(2 * i + hi) % (BWD ? W / 4 : 1)]) : act_pack(hid_act, lo_bits, hi_bits);
+							a[i / 2][(i & 1u) * 2 + hi] = v;
+							if (keep) *reinterpret_cast<uint32_t*>(keep + hi * 8 * W + 8 * i) = v;
+						}
 					}
 				} else {
-					// output layer: activation, then fp16 rows (and / or trimmed fp32 rows) to global memory. A full 64-column block
-					// goes out coalesced (transpose, then 8 lanes write 128 contiguous bytes of one row); a narrower tail row by row.
-					auto convert16 = [&](uint32_t c16, uint4& lo, uint4& hi) {
-						uint32_t r[16];
-						tmem_ld_n<16>(acc + c16 * 16, r);
-						tmem_ld_wait();
-						uint32_t y[8];
+					// output layer: activation, then fp16 rows (and / or trimmed fp32 rows) to global memory
 #pragma unroll
-						for (uint32_t i = 0; i < 8; ++i) {
-							const __half2 v = __halves2half2(act_fwd_h(out_act, __float2half_rn(__uint_as_float(r[2 * i]))), act_fwd_h(out_act, __float2half_rn(__uint_as_float(r[2 * i + 1]))));
-							y[i] = *reinterpret_cast<const uint32_t*>(&v);
-						}
-						lo = make_uint4(y[0], y[1], y[2], y[3]);
-						hi = make_uint4(y[4], y[5], y[6], y[7]);
-						if (p.output_fp32) {
+					for (uint32_t i = 0; i < C::ACC_N / 8; ++i) {
+						const uint32_t c = 8 * i + 2 * ft;
+						if (c >= last_w) continue;
 #pragma unroll
-							for (uint32_t i = 0; i < 16; ++i) {
-								const uint32_t col = c16 * 16 + i;
-								if (col < p.n_output_dims) p.output_fp32[sample * p.n_output_dims + col] = __half2float(reinterpret_cast<const __half*>(y)[i]);
+						for (uint32_t hi = 0; hi < 2; ++hi) {
+							const size_t rr = row0 + r0 + hi * 8;
+							const __half2 y = __halves2half2(act_fwd_h(out_act, __float2half_rn(acc[4 * i + 2 * hi])), act_fwd_h(out_act, __float2half_rn(acc[4 * i + 2 * hi + 1])));
+							if (p.output_fp16) *reinterpret_cast<__half2*>(p.output_fp16 + rr * last_w + c) = y;
+							if (p.output_fp32) {
+								if (c < p.n_output_dims) p.output_fp32[rr * p.n_output_dims + c] = __low2float(y);
+								if (c + 1 < p.n_output_dims) p.output_fp32[rr * p.n_output_dims + c + 1] = __high2float(y);
 							}
-						}
-					};
-					// this group's 16-column groups (one group per slot: all of the row -- dL/d(input) may be wider than the layers)
-					const uint32_t c16_begin = col0 / 16, c16_end = C::GROUPS == 1 ? (last_w + 15) / 16 : (col0 + C::GROUP_COLS) / 16;
-					uint32_t c16 = c16_begin;
-					if (C::GROUP_COLS == 64 && (c16 + 4) * 16 <= last_w) {
-						uint4 o[8];
-#pragma unroll
-						for (uint32_t q = 0; q < 4; ++q) convert16(c16 + q, o[2 * q], o[2 * q + 1]);
-						if (p.output_fp16) {
-							transpose8x8_u128(o, lane);
-#pragma unroll
-							for (uint32_t jj = 0; jj < 8; ++jj) *reinterpret_cast<uint4*>(p.output_fp16 + (tile_row0 + g8 * 8 + jj) * last_w + c16 * 16 + l8 * 8) = o[jj];
-						}
-						c16 += 4;
-					}
-					for (; c16 < c16_end && c16 * 16 < last_w; ++c16) {
-						uint4 lo, hi;
-						convert16(c16, lo, hi);
-						if (p.output_fp16) {
-							uint4* dst = reinterpret_cast<uint4*>(p.output_fp16 + sample * last_w + c16 * 16);
-							dst[0] = lo;
-							dst[1] = hi;
 						}
 					}
 				}
+				if (stamp) MLPF_STAMP(s, g, 3);
 			}
 		}
-		tc_fence_before_sync();
 	}
 
 	pdl_launch_dependents();
-	__syncthreads();
-	if (warp == C::EPI_WARPS) {
-		tc_fence_after_sync();
-		tmem_dealloc(tmem_base, C::TMEM_COLS);
-	}
 }
 
 // ------------------------------------------------------------------------------------------------------------------ host side
@@ -564,11 +298,11 @@ cudaError_t launch_impl(const MlpForwardParams& p, uint32_t n_sms, cudaStream_t 
 	w += (size_t)(p.n_hidden_layers - 1) * W * W;
 	if (!make_fp16_matrix_map(&mo, w, p.out_width, W, p.out_width)) return cudaErrorInvalidValue;
 	auto kernel = mlp_forward_kernel<W, GENERIC, BWD>;
-	const size_t smem = (size_t)kp.n_stages * C::STAGE_BYTES + 8 * (2 * MLPF_MAX_STAGES + 8) + 16;
+	const size_t smem = (size_t)kp.n_stages * C::STAGE_BYTES + 8 * 2 * MLPF_MAX_STAGES;
 	cudaError_t err = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
 	if (err != cudaSuccess) return err;
-	const uint32_t n_tiles = p.batch_size / TILE_M;
-	return launch_pdl(kernel, n_tiles < n_sms ? n_tiles : n_sms, C::THREADS, smem, stream, kp, m0, mh, mo);
+	const uint32_t n_groups = (p.batch_size / UNIT_M + C::WGS - 1) / C::WGS;  // CTAs that have a unit for every consumer warpgroup
+	return launch_pdl(kernel, n_groups < n_sms ? n_groups : n_sms, C::THREADS, smem, stream, kp, m0, mh, mo);
 }
 
 template <uint32_t W>

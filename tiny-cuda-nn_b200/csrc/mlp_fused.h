@@ -33,7 +33,7 @@ struct MlpForwardParams {
 	//   output_fp16 = dL/d(input) [batch][in_width] (may be null: the last step of the chain is then skipped).
 	uint32_t backward;
 	const __half* hidden_in;
-	// profiling only (scripts/mlp_timeline.py): clock64 stamps [cta][slot + 1 (0 = issuer)][64 events][8], null in production
+	// profiling only (tcnnb_network_debug_clocks): clock64 stamps [cta][consumer warpgroup (5 slots)][64 events][8], null in production
 	long long* dbg_clock;
 };
 

@@ -7,13 +7,13 @@
 //   * every CTA (one per SM) owns a contiguous range of 128-sample tiles and, for each tile and weight matrix, has TMA fetch the
 //     two operand tiles [128 samples][width] (SWIZZLE_128B boxes of 64 columns; narrower matrices are zero-filled by the TMA unit)
 //     into a ring of shared-memory stages;
-//   * both operands are read MN-major by tcgen05.mma (the batch is the K dimension: 8 steps of 16 samples per tile), accumulating
-//     fp32 in tensor memory for ALL tiles of the CTA: one [width][fan-in] accumulator per matrix, 512 columns = 4 matrices of 128 x 128
-//     or 8 of 64 x 64 per launch (deeper networks take several launches over disjoint matrices);
-//   * at the end each CTA adds its partial sums to the fp32 gradient accumulator with red.global.add.f32 (vectorised), which the
-//     optimizer consumes directly (Adam reads fp32 sums for the matrix parameters) or launch_mlp_grad_finalize casts to fp16.
+//   * both operands are read MN-major by wgmma (the batch is the K dimension: 8 steps of 16 samples per tile), accumulating fp32 in
+//     registers over all tiles of the CTA, one matrix after the other: M / 64 consumer warpgroups each own 64 rows of the
+//     [width][fan-in] accumulator;
+//   * at the end of a matrix each CTA adds its partial sums to the fp32 gradient accumulator with red.global.add.f32 (vectorised),
+//     which the optimizer consumes directly (Adam reads fp32 sums for the matrix parameters) or launch_mlp_grad_finalize casts to fp16.
 //
-// Warp roles: warp 0 = TMA producer, warp 1 = MMA issuer + TMEM allocation, warps 2..5 = flush (one per TMEM lane quadrant).
+// Warp roles: warpgroups 0 .. M / 64 - 1 = MMA + flush, the last warp = TMA producer.
 #include "mlp_fused.h"
 
 #include "fused_common.cuh"
@@ -31,19 +31,16 @@ namespace {
 template <uint32_t W>
 struct WgradCfg {
 	static constexpr uint32_t M = W == 128 ? 128 : 64;          // rows of an accumulator (narrower layers are zero-padded by TMA)
+	static constexpr uint32_t WGS = M / 64;                     // consumer warpgroups, 64 accumulator rows each
 	static constexpr uint32_t KB = (W + 63) / 64;               // 64-column boxes per operand tile
 	static constexpr uint32_t OPERAND_BYTES = KB * TILE_BYTES;
 	static constexpr uint32_t STAGE_BYTES = 2 * OPERAND_BYTES;  // [A | B]
 	static constexpr uint32_t STAGES = (200u * 1024u) / STAGE_BYTES < 8 ? (200u * 1024u) / STAGE_BYTES : 8;
-	static constexpr uint32_t THREADS = 6 * 32;
+	static constexpr uint32_t THREADS = WGS * 128 + 32;
 };
 
-constexpr uint32_t WGRAD_MAX_MATRICES = 16;
 struct WgradKernelParams {
 	MlpWgradParams p;
-	uint32_t first_matrix, n_matrices;  // this launch: matrices [first, first + n)
-	uint32_t tmem_cols;
-	uint16_t acc_col[WGRAD_MAX_MATRICES];  // first TMEM column of each matrix's accumulator (packed by the matrices' real fan-in)
 };
 
 }  // namespace
@@ -60,50 +57,41 @@ mlp_wgrad_kernel(const WgradKernelParams kp, const __grid_constant__ CUtensorMap
 	const uint32_t lane = tid & 31u;
 	const uint32_t NH = p.n_hidden_layers;
 	const uint32_t in_w = p.in_width, out_w = p.out_width;
+	const uint32_t n_matrices = NH + 1;
 
 	const uint32_t smem_base = smem_u32(smem_raw);
 	if (smem_base & 1023u) __trap();
 	const uint32_t s_bars = smem_base + C::STAGES * C::STAGE_BYTES;
 	const uint32_t bar_full = s_bars;                    // [STAGES] TMA complete_tx
-	const uint32_t bar_free = bar_full + 8 * C::STAGES;  // [STAGES] tcgen05.commit
-	const uint32_t bar_done = bar_free + 8 * C::STAGES;  // all MMAs of the CTA complete
-	const uint32_t s_tmem_slot = bar_done + 8;
+	const uint32_t bar_free = bar_full + 8 * C::STAGES;  // [STAGES] one arrival per consumer warp
 
 	if (tid == 0) {
 		for (uint32_t i = 0; i < C::STAGES; ++i) {
 			mbar_init(bar_full + 8 * i, 1);
-			mbar_init(bar_free + 8 * i, 1);
+			mbar_init(bar_free + 8 * i, C::WGS * 4);
 		}
-		mbar_init(bar_done, 1);
 		fence_mbar_init();
 	}
-	if (warp == 1) {
-		__syncwarp();
-		tmem_alloc(s_tmem_slot, kp.tmem_cols);
-		tmem_relinquish();
-	}
-	if (warp == 0 && lane == 0) {
+	if (warp == C::WGS * 4 && lane == 0) {
 		tma_prefetch_desc(&map_x);
 		tma_prefetch_desc(&map_h);
 		tma_prefetch_desc(&map_g);
 		tma_prefetch_desc(&map_go);
 	}
-	tc_fence_before_sync();
 	__syncthreads();
-	tc_fence_after_sync();
 	pdl_wait();
 
-	uint32_t tmem_base;
-	asm volatile("ld.shared.b32 %0, [%1];" : "=r"(tmem_base) : "r"(s_tmem_slot));
 	const uint32_t n_tiles = p.batch_size / TILE_M;
 	const uint32_t tile_begin = (uint32_t)((uint64_t)blockIdx.x * n_tiles / gridDim.x), tile_end = (uint32_t)((uint64_t)(blockIdx.x + 1) * n_tiles / gridDim.x);
-	const uint32_t n_items = (tile_end - tile_begin) * kp.n_matrices;  // (tile, matrix) pairs, matrix fastest
+	const uint32_t n_my = tile_end - tile_begin;
+	const uint32_t n_items = n_my * n_matrices;  // (matrix, tile) pairs, tile fastest
+	auto b_cols_of = [&](uint32_t mi) { return mi == 0 ? in_w : (mi == NH ? out_w : W); };
 
-	if (warp == 0) {
+	if (warp == C::WGS * 4) {
 		// =================================================================================== TMA producer
 		if (lane == 0) {
 			for (uint32_t it = 0; it < n_items; ++it) {
-				const uint32_t tile = tile_begin + it / kp.n_matrices, mi = kp.first_matrix + it % kp.n_matrices;
+				const uint32_t mi = it / n_my, tile = tile_begin + it % n_my;
 				const uint32_t stage = it % C::STAGES;
 				if (it >= C::STAGES) mbar_wait(bar_free + 8 * stage, ((it / C::STAGES) - 1u) & 1u);
 				const uint32_t a_dst = smem_base + stage * C::STAGE_BYTES, b_dst = a_dst + C::OPERAND_BYTES;
@@ -111,8 +99,7 @@ mlp_wgrad_kernel(const WgradKernelParams kp, const __grid_constant__ CUtensorMap
 				const int32_t row = (int32_t)(tile * TILE_M);
 				// matrix mi < NH: A = g_mi, B = h_{mi-1} (the network input for mi == 0);   output matrix: A = h_{NH-1}, B = dL/d(output)
 				// (transposed product: the accumulator's 128 / 64 rows are the layer's neurons either way)
-				const uint32_t b_cols = mi == 0 ? in_w : (mi == NH ? out_w : W);
-				const uint32_t b_boxes = (b_cols + 63) / 64;
+				const uint32_t b_boxes = (b_cols_of(mi) + 63) / 64;
 				mbar_arrive_expect_tx(full, (C::KB + b_boxes) * TILE_BYTES);
 				for (uint32_t b = 0; b < C::KB; ++b) {
 					if (mi < NH) tma_load_2d(a_dst + b * TILE_BYTES, &map_g, full, (int32_t)(b * 64), (int32_t)(mi * p.batch_size) + row);
@@ -125,67 +112,58 @@ mlp_wgrad_kernel(const WgradKernelParams kp, const __grid_constant__ CUtensorMap
 				}
 			}
 		}
-	} else if (warp == 1) {
-		// =================================================================================== MMA issuer
+	} else {
+		// =================================================================================== consumer warpgroup h: accumulator rows 64 h ..
+		const uint32_t h = warp / 4, wq = warp & 3u;
+		const uint32_t fq = lane >> 2, ft = lane & 3u;
+		constexpr uint32_t NMAX = C::KB * 64;  // widest fan-in
+		float d[NMAX / 2];
 		for (uint32_t it = 0; it < n_items; ++it) {
-			const uint32_t mi = kp.first_matrix + it % kp.n_matrices;
+			const uint32_t mi = it / n_my;
+			const bool first_tile = it % n_my == 0, last_tile = it % n_my == n_my - 1;
 			const uint32_t stage = it % C::STAGES;
+			const uint32_t n_cols = b_cols_of(mi);
 			mbar_wait(bar_full + 8 * stage, (it / C::STAGES) & 1u);
-			tc_fence_after_sync();
-			if (elect_one_sync()) {
-				const uint32_t a_tile = smem_base + stage * C::STAGE_BYTES, b_tile = a_tile + C::OPERAND_BYTES;
-				const uint32_t n_cols = mi == 0 ? in_w : (mi == NH ? out_w : W);
-				const uint32_t idesc = umma_idesc_f16(C::M, n_cols, 1, 1);
-				const uint32_t d_tmem = tmem_base + kp.acc_col[it % kp.n_matrices];
-				const bool first_tile = it < kp.n_matrices;
-				for (uint32_t kk = 0; kk < TILE_M / 16; ++kk) {
-					// [128 K-rows][64 MN] boxes: 16 K-rows per step = 2 048 bytes; the next 64 MN elements are one box (TILE_BYTES) further
-					const uint64_t a_desc = umma_desc_sw128(a_tile + kk * 2048u, TILE_BYTES, 1024u);
-					const uint64_t b_desc = umma_desc_sw128(b_tile + kk * 2048u, TILE_BYTES, 1024u);
-					umma_f16_ss(d_tmem, a_desc, b_desc, idesc, (!first_tile || kk > 0) ? 1u : 0u);
-				}
-				umma_commit(bar_free + 8 * stage);
-				if (it + 1 == n_items) umma_commit(bar_done);
+			const uint32_t a_tile = smem_base + stage * C::STAGE_BYTES + h * TILE_BYTES, b_tile = smem_base + stage * C::STAGE_BYTES + C::OPERAND_BYTES;
+			wgmma_fence();
+#pragma unroll
+			for (uint32_t kk = 0; kk < TILE_M / 16; ++kk) {
+				// [128 K-rows][64 MN] boxes: 16 K-rows per step = 2 048 bytes; the next 64 MN elements are one box (TILE_BYTES) further
+				const uint64_t a_desc = wgmma_desc_sw128(a_tile + kk * 2048u, TILE_BYTES, 1024u);
+				const uint64_t b_desc = wgmma_desc_sw128(b_tile + kk * 2048u, TILE_BYTES, 1024u);
+				const uint32_t acc = (!first_tile || kk > 0) ? 1u : 0u;
+				if (NMAX == 128 && n_cols > 64) Wgmma<NMAX>::template ss<1, 1>(reinterpret_cast<float(&)[NMAX / 2]>(d), a_desc, b_desc, acc);
+				else Wgmma<64>::template ss<1, 1>(reinterpret_cast<float(&)[32]>(d), a_desc, b_desc, acc);
 			}
+			wgmma_commit();
+			wgmma_wait<0>();
+			reg_fence(d);
 			__syncwarp();
-		}
-	} else if (n_items) {
-		// =================================================================================== flush: partial sums -> global fp32
-		mbar_wait(bar_done, 0);
-		tc_fence_after_sync();
-		const uint32_t quad = warp & 3u;  // a warp reads the TMEM lane quadrant (warp index mod 4)
-		const uint32_t lane_field = (quad * 32u) << 16;
-		// accumulator row of this thread: M = 128 -> lane index; M = 64 -> lanes 0..15 of each quadrant hold rows 16 quad + lane
-		const uint32_t m = C::M == 128 ? quad * 32 + lane : quad * 16 + lane;
-		const bool row_ok = (C::M == 128 || lane < 16) && m < W;
-		for (uint32_t a = 0; a < kp.n_matrices; ++a) {
-			const uint32_t mi = kp.first_matrix + a;
-			const uint32_t n_cols = mi == 0 ? in_w : (mi == NH ? out_w : W);
+			if (lane == 0) mbar_arrive_plain(bar_free + 8 * stage);
+			if (!last_tile) continue;
+			// ---- flush: partial sums -> global fp32. d[4 i + q]: row m = 64 h + 16 wq + lane / 4 (+ 8 for q >= 2), column 8 i + 2 (lane % 4) + (q & 1)
 			float* base = p.dw_accum + (mi == 0 ? 0 : (size_t)W * in_w + (size_t)(mi - 1) * W * W);
-			for (uint32_t c0 = 0; c0 < n_cols; c0 += 16) {
-				uint32_t r[16];
-				tmem_ld_32x32b_x16(tmem_base + lane_field + kp.acc_col[a] + c0, r);
-				tmem_ld_wait();
-				if (!row_ok) continue;
-				if (mi < NH) {
-					float* dst = base + (size_t)m * n_cols + c0;  // W_mi[m][c0 ..]
 #pragma unroll
-					for (uint32_t q = 0; q < 16; q += 4) red_add_v4_f32(dst + q, __uint_as_float(r[q]), __uint_as_float(r[q + 1]), __uint_as_float(r[q + 2]), __uint_as_float(r[q + 3]));
-				} else {
+			for (uint32_t i = 0; i < NMAX / 8; ++i) {
+				const uint32_t n = 8 * i + 2 * ft;
+				if (n >= n_cols) continue;
 #pragma unroll
-					for (uint32_t q = 0; q < 16; ++q) red_add_f32(base + (size_t)(c0 + q) * W + m, __uint_as_float(r[q]));  // W_out[c0 + q][m]
+				for (uint32_t hi = 0; hi < 2; ++hi) {
+					const uint32_t m = h * 64 + wq * 16 + fq + hi * 8;
+					if (m >= W) continue;
+					const float v0 = d[4 * i + 2 * hi], v1 = d[4 * i + 2 * hi + 1];
+					if (mi < NH) {
+						red_add_v2_f32(base + (size_t)m * n_cols + n, v0, v1);  // W_mi[m][n ..]
+					} else {
+						red_add_f32(base + (size_t)n * W + m, v0);  // W_out[n][m]
+						red_add_f32(base + (size_t)(n + 1) * W + m, v1);
+					}
 				}
 			}
 		}
-		tc_fence_before_sync();
 	}
 
 	pdl_launch_dependents();
-	__syncthreads();
-	if (warp == 1) {
-		tc_fence_after_sync();
-		tmem_dealloc(tmem_base, kp.tmem_cols);
-	}
 }
 
 namespace {
@@ -200,33 +178,15 @@ cudaError_t launch_wgrad_width(const MlpWgradParams& p, uint32_t n_sms, cudaStre
 	if (!make_fp16_matrix_map(&mg, p.grad_hidden, (uint64_t)NH * B, W, TILE_M)) return cudaErrorInvalidValue;
 	if (!make_fp16_matrix_map(&mgo, p.grad_output, B, p.out_width, TILE_M)) return cudaErrorInvalidValue;
 	auto kernel = mlp_wgrad_kernel<W>;
-	const size_t smem = (size_t)C::STAGES * C::STAGE_BYTES + 8 * (2 * C::STAGES + 1) + 16;
+	const size_t smem = (size_t)C::STAGES * C::STAGE_BYTES + 8 * 2 * C::STAGES;
 	cudaError_t err = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
 	if (err != cudaSuccess) return err;
 	const uint32_t n_tiles = B / TILE_M;
-	const uint32_t n_matrices = NH + 1;
-	// accumulators are packed by the matrices' real column counts (fan-in; 16-column granules): 128 x 4 with a 32-wide input and 16
-	// outputs needs 32 + 3 x 128 + 16 = 432 of the 512 columns -- one launch
-	auto cols_of = [&](uint32_t mi) { return ((mi == 0 ? p.in_width : (mi == NH ? p.out_width : W)) + 15u) / 16u * 16u; };
-	for (uint32_t first = 0; first < n_matrices;) {
-		WgradKernelParams kp{};
-		kp.p = p;
-		kp.first_matrix = first;
-		uint32_t used = 0, n = 0;
-		while (first + n < n_matrices && n < WGRAD_MAX_MATRICES && used + cols_of(first + n) <= 512) {
-			kp.acc_col[n] = (uint16_t)used;
-			used += cols_of(first + n);
-			++n;
-		}
-		kp.n_matrices = n;
-		uint32_t cols = 32;
-		while (cols < used) cols *= 2;
-		kp.tmem_cols = cols;
-		err = launch_pdl(kernel, n_tiles < n_sms ? n_tiles : n_sms, C::THREADS, smem, stream, kp, mx, mh, mg, mgo);
-		if (err != cudaSuccess) return err;
-		if (n_launches) ++*n_launches;
-		first += n;
-	}
+	WgradKernelParams kp{};
+	kp.p = p;
+	err = launch_pdl(kernel, n_tiles < n_sms ? n_tiles : n_sms, C::THREADS, smem, stream, kp, mx, mh, mg, mgo);
+	if (err != cudaSuccess) return err;
+	if (n_launches) ++*n_launches;
 	return cudaSuccess;
 }
 

@@ -142,7 +142,7 @@ struct Model {
 	const __half* inference_params() const { return ema.enabled ? ema_fp16.ptr : params_fp16; }
 	float loss_scale = 128.0f;  // default_loss_scale<__half>() (common.h:243)
 	int device = 0;
-	int n_sms = 148;
+	int n_sms = 132;
 
 	size_t n_params = 0;
 	// trainer.h:489-503: one allocation [fp32 master | fp16 params | fp16 gradients]
@@ -291,8 +291,8 @@ static void build_model(Model& m, uint32_t n_in, uint32_t n_out, const json::Val
 	TCNNB_CUDA_CHECK(cudaGetDevice(&m.device));
 	cudaDeviceProp prop;
 	TCNNB_CUDA_CHECK(cudaGetDeviceProperties(&prop, m.device));
-	if (prop.major != 10) {
-		throw std::runtime_error("tcnn_b200 requires an sm_100-class GPU (B200); found compute capability " + std::to_string(prop.major) + "." + std::to_string(prop.minor));
+	if (prop.major != 9) {
+		throw std::runtime_error("tcnn_b200 requires an sm_90-class GPU (H100); found compute capability " + std::to_string(prop.major) + "." + std::to_string(prop.minor));
 	}
 	m.n_sms = prop.multiProcessorCount;
 #ifdef TCNNB_ENABLE_ABLATION  // profiling builds only (make ABLATION=1); the production library reads no environment switches

@@ -27,7 +27,7 @@ struct Network {
 	uint32_t padded_out_width = 0;
 	uint32_t activation = ACT_RELU, output_activation = ACT_NONE;
 	uint64_t n_params = 0;
-	int n_sms = 148;
+	int n_sms = 132;
 	long long* dbg_clock = nullptr;  // profiling only (tcnnb_network_debug_clocks)
 	std::string otype, hyperparams_json;
 	// scratch of the backward pass (grown on demand, reused): g_l rows, dL/d(output) through the output activation, fp32 weight-gradient
@@ -41,7 +41,7 @@ static void build_network(Network& n, uint32_t n_in, uint32_t n_out, const json:
 	TCNNB_CUDA_CHECK(cudaGetDevice(&device));
 	cudaDeviceProp prop;
 	TCNNB_CUDA_CHECK(cudaGetDeviceProperties(&prop, device));
-	if (prop.major != 10) throw std::runtime_error("tcnn_b200 requires an sm_100-class GPU (B200); found compute capability " + std::to_string(prop.major) + "." + std::to_string(prop.minor));
+	if (prop.major != 9) throw std::runtime_error("tcnn_b200 requires an sm_90-class GPU (H100); found compute capability " + std::to_string(prop.major) + "." + std::to_string(prop.minor));
 	n.n_sms = prop.multiProcessorCount;
 	n.otype = net.value("otype", "MLP");  // src/network.cu:52-54
 	const bool fully_fused = ieq(n.otype, "FullyFusedMLP") || ieq(n.otype, "MegakernelMLP");
@@ -51,7 +51,7 @@ static void build_network(Network& n, uint32_t n_in, uint32_t n_out, const json:
 	n.n_hidden_layers = (uint32_t)net.value("n_hidden_layers", 5.0);
 	n.activation = parse_activation(net.value("activation", "ReLU"));
 	n.output_activation = parse_activation(net.value("output_activation", "None"));
-	// Both otypes run on the same tcgen05 kernel (there is no separate non-fused path in this library), so both take the fused
+	// Both otypes run on the same wgmma kernel (there is no separate non-fused path in this library), so both take the fused
 	// kernel's widths; the reference's CutlassMLP accepts any multiple of 8.
 	if (!(n.width == 16 || n.width == 32 || n.width == 64 || n.width == 128)) {
 		throw std::runtime_error("FullyFusedMLP only supports 16, 32, 64, and 128 neurons, but got " + std::to_string(n.width) + ". Use CutlassMLP instead if this is a requirement.");

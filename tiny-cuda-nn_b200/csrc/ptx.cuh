@@ -1,6 +1,6 @@
-// ptx.cuh -- thin inline-PTX wrappers for the sm_100a features the kernels use:
-// mbarrier, tcgen05 (alloc / mma / commit / ld / fences), async-proxy fences, f16x2 reductions.
-// Everything here is sm_100a-only by design (no fallback paths).
+// ptx.cuh -- thin inline-PTX wrappers for the sm_90a features the kernels use:
+// mbarrier, wgmma (warpgroup MMA, shared-memory descriptors), async-proxy fences, TMA, f16x2 / f32 reductions.
+// Everything here is sm_90a-only by design (no fallback paths).
 #pragma once
 #include <cuda_fp16.h>
 #include <stdint.h>
@@ -35,163 +35,137 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
 }
 
 // ---------------------------------------------------------------- proxies / fences
-// Make generic-proxy shared-memory writes visible to the async proxy (tcgen05.mma operand reads).
+// Make generic-proxy shared-memory writes visible to the async proxy (wgmma operand reads).
 __device__ __forceinline__ void fence_proxy_async_smem() {
 	asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
 
-__device__ __forceinline__ void tc_fence_before_sync() {
-	asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-
-__device__ __forceinline__ void tc_fence_after_sync() {
-	asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-
-// ---------------------------------------------------------------- TMEM allocation (one full warp calls these)
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_dst, uint32_t n_cols) {
-	asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(n_cols) : "memory");
-}
-
-__device__ __forceinline__ void tmem_relinquish() {
-	asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t n_cols) {
-	asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(n_cols) : "memory");
-}
-
-// ---------------------------------------------------------------- UMMA descriptors
+// ---------------------------------------------------------------- wgmma
 // Shared-memory matrix descriptor, SWIZZLE_128B canonical layouts (tile rows are 128 bytes = 64 fp16):
 //   bits [ 0,14) start address >> 4        bits [16,30) leading byte offset >> 4
-//   bits [32,46) stride byte offset >> 4   bits [46,48) version = 1 (sm_100)
-//   bits [61,64) layout type: 2 = SWIZZLE_128B
-// K-major operand  ([rows = M/N][64 K-elements]):  SBO = 1024 B (next group of 8 rows), LBO unused (1).
+//   bits [32,46) stride byte offset >> 4   bits [62,64) layout type: 1 = SWIZZLE_128B
+// K-major operand  ([rows = M/N][64 K-elements]):  SBO = 1024 B (next group of 8 rows), LBO unused (1); the k-th step of 16 elements
+//   starts 32 k bytes into the row (the hardware applies the swizzle to the computed addresses).
 // MN-major operand ([rows = K][64 MN-elements]):   SBO = 1024 B (next group of 8 K-rows), LBO = stride between
 //   64-element blocks along MN (only read when the MN extent exceeds 64).
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
 	uint64_t d = 0;
 	d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
 	d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
 	d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-	d |= (uint64_t)1 << 46;
-	d |= (uint64_t)2 << 61;
+	d |= (uint64_t)1 << 62;
 	return d;
 }
 
-// Instruction descriptor for kind::f16 with fp16 A/B and fp32 accumulation.
-//   [4,6) c_format = 1 (f32); [7,10) a_format = 0 (f16); [10,13) b_format = 0 (f16);
-//   [15] a_major (0 = K, 1 = MN); [16] b_major; [17,23) N >> 3; [24,29) M >> 4.
-__host__ __device__ constexpr uint32_t umma_idesc_f16(uint32_t M, uint32_t N, uint32_t a_mn_major, uint32_t b_mn_major) {
-	return (1u << 4) | (a_mn_major << 15) | (b_mn_major << 16) | ((N >> 3) << 17) | ((M >> 4) << 24);
+// Orders the warpgroup's register / shared-memory accesses before the wgmma instructions that follow.
+__device__ __forceinline__ void wgmma_fence() {
+	asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
 }
 
-// D[tmem] (+)= A[smem] * B[smem], issued by ONE thread.
-__device__ __forceinline__ void umma_f16_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-	asm volatile(
-		"{\n"
-		".reg .pred p;\n"
-		"setp.ne.b32 p, %4, 0;\n"
-		"tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-		"}\n" ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-		: "memory");
+__device__ __forceinline__ void wgmma_commit() {
+	asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
 }
 
-// One lane of a converged warp (elect.sync). With a warp-UNIFORM enclosing branch this lets the compiler keep the operands of the
-// tcgen05 instructions in uniform registers; under a `tid == 0` branch it wraps every UTCHMMA in an ELECT / R2UR loop instead.
-__device__ __forceinline__ bool elect_one_sync() {
-	uint32_t pred;
-	asm volatile(
-		"{\n"
-		".reg .pred p;\n"
-		"elect.sync _|p, 0xffffffff;\n"
-		"selp.u32 %0, 1, 0, p;\n"
-		"}\n"
-		: "=r"(pred));
-	return pred != 0;
+// Wait until at most N committed groups of this warp are pending.
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+	asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
 
-// Arrive on an mbarrier once all previously issued tcgen05.mma of this thread have completed.
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-	asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
+// Pins the accumulator registers at this point of the program: the compiler must not move their reads above a wgmma_wait.
+template <int R>
+__device__ __forceinline__ void reg_fence(float (&d)[R]) {
+#pragma unroll
+	for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// ---------------------------------------------------------------- TMEM -> registers
-// 32x32b: lane i of the warp reads TMEM lane (base_lane + i); .x32 = 32 consecutive 32-bit columns.
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
-	asm volatile(
-		"tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-		"{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-		"%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-		: "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-		  "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-		  "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-		  "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-		: "r"(taddr)
-		: "memory");
-}
+// D[64 x N] (+)= A[64 x 16] . B[16 x N], fp16 operands, fp32 accumulators in registers (scale_d = 0: D is overwritten).
+//   ss: A and B from shared memory (descriptors); TA / TB = 1: the operand is MN-major (transposed).
+//   rs: A from registers in the accumulator-compatible fragment layout (thread (warp w, lane l) holds rows 16 w + l / 4 and + 8,
+//       columns 2 (l % 4) + {0, 1} and + 8, as packed fp16 pairs a[0..3] = (r, c), (r + 8, c), (r, c + 8), (r + 8, c + 8)).
+// Accumulator fragment: d[4 i + {0, 1}] = row 16 w + l / 4, columns 8 i + 2 (l % 4) + {0, 1}; d[4 i + {2, 3}] = the row 8 below.
+template <int N>
+struct Wgmma;
 
-__device__ __forceinline__ void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t (&r)[16]) {
-	asm volatile(
-		"tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-		"{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-		: "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-		  "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-		: "r"(taddr)
-		: "memory");
-}
+template <>
+struct Wgmma<16> {
+	template <int TA, int TB>
+	__device__ __forceinline__ static void ss(float (&d)[8], uint64_t a, uint64_t b, uint32_t scale_d) {
+		asm volatile(
+			"{\n.reg .pred p;\nsetp.ne.b32 p, %10, 0;\n"
+			"wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, %11, %12;\n}\n"
+			: "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+			: "l"(a), "l"(b), "r"(scale_d), "n"(TA), "n"(TB));
+	}
+	template <int TB>
+	__device__ __forceinline__ static void rs(float (&d)[8], const uint32_t (&a)[4], uint64_t b, uint32_t scale_d) {
+		asm volatile(
+			"{\n.reg .pred p;\nsetp.ne.b32 p, %13, 0;\n"
+			"wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1, %14;\n}\n"
+			: "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+			: "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(scale_d), "n"(TB));
+	}
+};
 
-__device__ __forceinline__ void tmem_ld_wait() {
-	asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
+template <>
+struct Wgmma<32> {
+	template <int TA, int TB>
+	__device__ __forceinline__ static void ss(float (&d)[16], uint64_t a, uint64_t b, uint32_t scale_d) {
+		asm volatile(
+			"{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+			"wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, %19, %20;\n}\n"
+			: "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+			: "l"(a), "l"(b), "r"(scale_d), "n"(TA), "n"(TB));
+	}
+	template <int TB>
+	__device__ __forceinline__ static void rs(float (&d)[16], const uint32_t (&a)[4], uint64_t b, uint32_t scale_d) {
+		asm volatile(
+			"{\n.reg .pred p;\nsetp.ne.b32 p, %21, 0;\n"
+			"wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p, 1, 1, %22;\n}\n"
+			: "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+			: "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(scale_d), "n"(TB));
+	}
+};
 
+template <>
+struct Wgmma<64> {
+	template <int TA, int TB>
+	__device__ __forceinline__ static void ss(float (&d)[32], uint64_t a, uint64_t b, uint32_t scale_d) {
+		asm volatile(
+			"{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+			"wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, %36;\n}\n"
+			: "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+			: "l"(a), "l"(b), "r"(scale_d), "n"(TA), "n"(TB));
+	}
+	template <int TB>
+	__device__ __forceinline__ static void rs(float (&d)[32], const uint32_t (&a)[4], uint64_t b, uint32_t scale_d) {
+		asm volatile(
+			"{\n.reg .pred p;\nsetp.ne.b32 p, %37, 0;\n"
+			"wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, %38;\n}\n"
+			: "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+			: "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(scale_d), "n"(TB));
+	}
+};
 
-// ---------------------------------------------------------------- more TMEM <-> register shapes (stand-alone MLP kernel)
-__device__ __forceinline__ void tmem_ld_32x32b_x64(uint32_t taddr, uint32_t (&r)[64]) {
-	asm volatile("tcgen05.ld.sync.aligned.32x32b.x64.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, [%64];"
-		: "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31]), "=r"(r[32]), "=r"(r[33]), "=r"(r[34]), "=r"(r[35]), "=r"(r[36]), "=r"(r[37]), "=r"(r[38]), "=r"(r[39]), "=r"(r[40]), "=r"(r[41]), "=r"(r[42]), "=r"(r[43]), "=r"(r[44]), "=r"(r[45]), "=r"(r[46]), "=r"(r[47]), "=r"(r[48]), "=r"(r[49]), "=r"(r[50]), "=r"(r[51]), "=r"(r[52]), "=r"(r[53]), "=r"(r[54]), "=r"(r[55]), "=r"(r[56]), "=r"(r[57]), "=r"(r[58]), "=r"(r[59]), "=r"(r[60]), "=r"(r[61]), "=r"(r[62]), "=r"(r[63])
-		: "r"(taddr)
-		: "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x32b_x8(uint32_t taddr, uint32_t (&r)[8]) {
-	asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-		: "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-		: "r"(taddr)
-		: "memory");
-}
-
-// registers -> TMEM, 32x32b: lane i of the warp writes TMEM lane (base_lane + i), n consecutive 32-bit columns.
-__device__ __forceinline__ void tmem_st_32x32b_x8(uint32_t taddr, const uint32_t (&r)[8]) {
-	asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%8], {%0, %1, %2, %3, %4, %5, %6, %7};"
-		:: "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(taddr)
-		: "memory");
-}
-__device__ __forceinline__ void tmem_st_32x32b_x16(uint32_t taddr, const uint32_t (&r)[16]) {
-	asm volatile("tcgen05.st.sync.aligned.32x32b.x16.b32 [%16], {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15};"
-		:: "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(taddr)
-		: "memory");
-}
-__device__ __forceinline__ void tmem_st_32x32b_x32(uint32_t taddr, const uint32_t (&r)[32]) {
-	asm volatile("tcgen05.st.sync.aligned.32x32b.x32.b32 [%32], {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31};"
-		:: "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31]), "r"(taddr)
-		: "memory");
-}
-
-__device__ __forceinline__ void tmem_st_wait() {
-	asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-}
-
-// D[tmem] (+)= A[tmem] * B[smem]: the A operand (M rows <-> TMEM lanes, K along the columns, two fp16 per 32-bit column) is read
-// from tensor memory -- the previous layer's activations never pass through shared memory.
-__device__ __forceinline__ void umma_f16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-	asm volatile(
-		"{\n"
-		".reg .pred p;\n"
-		"setp.ne.b32 p, %4, 0;\n"
-		"tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n"
-		"}\n" ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-		: "memory");
-}
+template <>
+struct Wgmma<128> {
+	template <int TA, int TB>
+	__device__ __forceinline__ static void ss(float (&d)[64], uint64_t a, uint64_t b, uint32_t scale_d) {
+		asm volatile(
+			"{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+			"wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, %67, %68;\n}\n"
+			: "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+			: "l"(a), "l"(b), "r"(scale_d), "n"(TA), "n"(TB));
+	}
+	template <int TB>
+	__device__ __forceinline__ static void rs(float (&d)[64], const uint32_t (&a)[4], uint64_t b, uint32_t scale_d) {
+		asm volatile(
+			"{\n.reg .pred p;\nsetp.ne.b32 p, %69, 0;\n"
+			"wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, {%64, %65, %66, %67}, %68, p, 1, 1, %70;\n}\n"
+			: "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+			: "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(scale_d), "n"(TB));
+	}
+};
 
 // ---------------------------------------------------------------- mbarrier extras + TMA (cp.async.bulk.tensor)
 __device__ __forceinline__ bool mbar_test(uint32_t bar, uint32_t parity) {
@@ -237,7 +211,11 @@ __device__ __forceinline__ void red_add_f32(float* addr, float v) {
 	asm volatile("red.relaxed.gpu.global.add.f32 [%0], %1;" ::"l"(addr), "f"(v) : "memory");
 }
 
-// 16-byte vector reduction (sm_90+): four fp32 adds in one L2 operation; address must be 16-byte aligned.
+// 8- / 16-byte vector reductions (sm_90+): two / four fp32 adds in one L2 operation; the address must be 8- / 16-byte aligned.
+__device__ __forceinline__ void red_add_v2_f32(float* addr, float a, float b) {
+	asm volatile("red.relaxed.gpu.global.add.v2.f32 [%0], {%1, %2};" ::"l"(addr), "f"(a), "f"(b) : "memory");
+}
+
 __device__ __forceinline__ void red_add_v4_f32(float* addr, float a, float b, float c, float d) {
 	asm volatile("red.relaxed.gpu.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
 }

@@ -4,7 +4,7 @@ This mirrors, in Python, the names a user of the reference touches on this path:
 `create_from_config(n_input_dims, n_output_dims, config)` -> TrainableModel with `.trainer.training_step(...)`,
 `.trainer.loss()`, `.network.inference(...)` (config.h:46-63, trainer.h:254-378, object.h:214).
 It is plumbing for tests and bench.py: torch is used only for device memory and streams. There is no CPU
-fallback -- if the CUDA library is missing or the device is not a B200, construction raises.
+fallback -- if the CUDA library is missing or the device is not an sm_90 (H100-class) GPU, construction raises.
 """
 import ctypes
 import json

@@ -14,7 +14,7 @@ backward pass and the parameter / input gradients divided by it afterwards (modu
 sliced away (modules.py:233). Gradients w.r.t. the input positions are delivered when the input requires grad (modules.py:153-160).
 Not supported: second-order terms (bwd_bwd_input).
 
-This file is glue: the work happens in libtcnn_b200 (fused sm_100a kernels) behind `tcnnb_module_*`, `tcnnb_encoding_*`, `tcnnb_network_*`.
+This file is glue: the work happens in libtcnn_b200 (fused sm_90a kernels) behind `tcnnb_module_*`, `tcnnb_encoding_*`, `tcnnb_network_*`.
 """
 import torch
 
