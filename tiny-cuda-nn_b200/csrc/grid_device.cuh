@@ -238,9 +238,18 @@ __device__ __forceinline__ void level_corners(const LevelInfo& lv, const float (
 // keep several levels of loads in flight, and anything that touches a value -- an earlier version fetched the aligned 8-byte slot
 // and SELECTED the two halves -- makes the warp wait for the loads it has just issued (that version ran at a depth of one
 // level whatever the software pipeline said; scripts/ws_timeline.py: gather 10.2 -> see DESIGN.md section 3.1).
-__device__ __forceinline__ void gather_pair_f16x2(const uint32_t* __restrict__ table, uint32_t idx0, uint32_t idx1, bool /*paired*/, uint32_t& v0, uint32_t& v1) {
-	v0 = __ldg(table + idx0);
-	v1 = __ldg(table + idx1);
+// `streaming` (warp-uniform): the loads do not allocate in L1. The training kernel uses it for the hashed levels, whose entries
+// are spread at random over megabytes and are rarely met again by the same SM, so that the L1 (smaller in training: park and dy
+// tiles) is left to the dense coarse levels that neighbouring samples of the binned batch share. Measured in DESIGN.md 5.1.
+__device__ __forceinline__ uint32_t ld_table(const uint32_t* p, bool streaming) {
+	uint32_t v;
+	if (streaming) asm("ld.global.nc.L1::no_allocate.b32 %0, [%1];" : "=r"(v) : "l"(p));
+	else v = __ldg(p);
+	return v;
+}
+__device__ __forceinline__ void gather_pair_f16x2(const uint32_t* __restrict__ table, uint32_t idx0, uint32_t idx1, bool /*paired*/, bool streaming, uint32_t& v0, uint32_t& v1) {
+	v0 = ld_table(table + idx0, streaming);
+	v1 = ld_table(table + idx1, streaming);
 }
 
 // Scatter-add two fp16x2 addends of a corner pair (red.global.add.noftz.f16x2 is what the reference's
