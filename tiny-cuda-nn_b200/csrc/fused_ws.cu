@@ -287,38 +287,48 @@ __global__ void __launch_bounds__(WS_THREADS, 1) fused_ws_kernel(const FusedStep
 				// Three levels in flight: the loads of levels l+1 and l+2 are issued before the values of level l are consumed.
 				// What travels with the loads is the fractional position (D floats), not the 2^D weights: they are rebuilt at
 				// consumption, which is what makes the third level fit the register budget.
+				// issue() returns bit k set when pair k came back as one 8-byte slot with its words in the other order from corner
+				// order (gather_pair_f16x2); the bits of the three levels in flight travel together in one word, `swaps`, NP bits a level.
+				constexpr uint32_t NP = 1u << (D - 1);
 				struct InFlight {
 					uint32_t vals[1u << D];
 					float frac[D];
 				};
-				auto issue = [&](uint32_t level, InFlight& f) {
+				auto issue = [&](uint32_t level, InFlight& f) -> uint32_t {
 					const LevelInfo& lv = load_level(level);
 					LevelCorners<D> lc;
 					level_corners<D>(lv, x_cur, p.grid.interpolation, lc);
 					const uint32_t* __restrict__ ltab = reinterpret_cast<const uint32_t*>(table + (size_t)lv.offset * F);
 					// Training: the hashed levels' gathers do not allocate in L1 (headline step, H100 80GB HBM3 at 400 W: fused kernel
-					// 0.518 -> 0.483 ms). Inference keeps them in L1: streaming them there measured 0.168 -> 0.242 ms.
+					// 0.518 -> 0.483 ms), and a pair that shares an aligned slot is fetched with one 8-byte load. Inference keeps them
+					// in L1: streaming them there measured 0.168 -> 0.242 ms.
+					const bool streaming = TRAIN && lv.use_hash == LEVEL_HASH;
+					uint32_t swapped = 0;
 #pragma unroll
-					for (uint32_t pr = 0; pr < (1u << (D - 1)); ++pr) {
+					for (uint32_t pr = 0; pr < NP; ++pr) {
 						const bool paired = (lc.paired >> pr) & 1u;
 						if (TCNNB_ABLATE(ABLATE_GATHER) || (TCNNB_ABLATE(ABLATE_GATHER_DENSE) && lv.use_hash == 0) || (TCNNB_ABLATE(ABLATE_GATHER_HASH) && lv.use_hash != 0)) {
 							f.vals[2 * pr] = lc.idx[2 * pr];
 							f.vals[2 * pr + 1] = lc.idx[2 * pr + 1];
 						} else {
-							gather_pair_f16x2(ltab, lc.idx[2 * pr], lc.idx[2 * pr + 1], paired && !(TCNNB_ABLATE(ABLATE_PAIRING)), TRAIN && lv.use_hash == LEVEL_HASH, f.vals[2 * pr], f.vals[2 * pr + 1]);
+							const bool merge = streaming && lv.wide_ok && paired && !(TCNNB_ABLATE(ABLATE_PAIRING));
+							swapped |= gather_pair_f16x2(ltab, lc.idx[2 * pr], lc.idx[2 * pr + 1], merge, streaming, f.vals[2 * pr], f.vals[2 * pr + 1]) << pr;
 						}
 					}
 #pragma unroll
 					for (uint32_t d = 0; d < D; ++d) f.frac[d] = lc.frac[d];
+					return swapped;
 				};
-				auto consume = [&](uint32_t level, const InFlight& f) {
+				auto consume = [&](uint32_t level, const InFlight& f, uint32_t swapped) {
 					float w[1u << D];
 					corner_weights<D>(f.frac, w);
 					__half2 result = __float2half2_rn(0.0f);
 #pragma unroll
 					for (uint32_t idx = 0; idx < (1u << D); ++idx) {
+						const bool sw = (swapped >> (idx / 2)) & 1u;
+						const uint32_t v = sw ? f.vals[idx ^ 1u] : f.vals[idx];
 						// fma((T)weight, grid_val, result) with T = __half -> __hfma2 (grid.h:162, vec.h:372-378)
-						result = __hfma2(__float2half2_rn(w[idx]), *reinterpret_cast<const __half2*>(&f.vals[idx]), result);
+						result = __hfma2(__float2half2_rn(w[idx]), *reinterpret_cast<const __half2*>(&v), result);
 					}
 					const uint32_t feat = level * F;
 					asm volatile("st.shared.b32 [%0], %1;" ::"r"(enc_tile + sw128(row, feat >> 3) + (feat & 7u) * 2u), "r"(*reinterpret_cast<uint32_t*>(&result)) : "memory");
@@ -326,12 +336,13 @@ __global__ void __launch_bounds__(WS_THREADS, 1) fused_ws_kernel(const FusedStep
 				};
 				if (level_begin < level_end) {
 					InFlight f0, f1, f2;
-					issue(level_begin, f0);
-					if (level_begin + 1 < level_end) issue(level_begin + 1, f1);
+					uint32_t swaps = issue(level_begin, f0);
+					if (level_begin + 1 < level_end) swaps |= issue(level_begin + 1, f1) << NP;
 #pragma unroll 1
 					for (uint32_t level = level_begin; level < level_end; ++level) {
-						if (level + 2 < level_end) issue(level + 2, f2);
-						consume(level, f0);
+						if (level + 2 < level_end) swaps |= issue(level + 2, f2) << (2 * NP);
+						consume(level, f0, swaps);
+						swaps >>= NP;
 						f0 = f1;
 						f1 = f2;
 					}

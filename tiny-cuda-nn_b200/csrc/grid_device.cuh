@@ -233,8 +233,8 @@ __device__ __forceinline__ void level_corners(const LevelInfo& lv, const float (
 	}
 }
 
-// Gather the two fp16x2 entries of a corner pair: two independent 4-byte loads (for an aligned pair they fall into the same
-// 32-byte sector, so the second one costs no extra L2 traffic). Deliberately NO arithmetic on the loaded values here: callers
+// Gather the two fp16x2 entries of a corner pair: two independent 4-byte loads, or one 8-byte load (`merge`, below).
+// Deliberately NO arithmetic on the loaded values here: callers
 // keep several levels of loads in flight, and anything that touches a value -- an earlier version fetched the aligned 8-byte slot
 // and SELECTED the two halves -- makes the warp wait for the loads it has just issued (that version ran at a depth of one
 // level whatever the software pipeline said; scripts/ws_timeline.py: gather 10.2 -> see DESIGN.md section 3.1).
@@ -247,9 +247,19 @@ __device__ __forceinline__ uint32_t ld_table(const uint32_t* p, bool streaming) 
 	else v = __ldg(p);
 	return v;
 }
-__device__ __forceinline__ void gather_pair_f16x2(const uint32_t* __restrict__ table, uint32_t idx0, uint32_t idx1, bool /*paired*/, bool streaming, uint32_t& v0, uint32_t& v1) {
+// `merge`: the pair shares an aligned 8-byte slot (`paired`) and the level base is 16-byte aligned (LevelInfo::wide_ok). The
+// pair is then fetched with ONE 8-byte streaming load, which costs one L2 request instead of two (with L1 allocation the second
+// 4-byte load hit the sector the first had just brought in, so merging saved nothing; measured in DESIGN.md 5.1). The words
+// arrive in memory order, v0 = entry (idx0 & ~1): the return value is 1 when they are the other way round from corner order
+// (idx0 odd -- the hash XORs the x bit with the other coordinates' bits), and the caller swaps them when it consumes them.
+__device__ __forceinline__ uint32_t gather_pair_f16x2(const uint32_t* __restrict__ table, uint32_t idx0, uint32_t idx1, bool merge, bool streaming, uint32_t& v0, uint32_t& v1) {
+	if (merge) {
+		asm("ld.global.nc.L1::no_allocate.v2.b32 {%0, %1}, [%2];" : "=r"(v0), "=r"(v1) : "l"(table + (idx0 & ~1u)));
+		return idx0 & 1u;
+	}
 	v0 = ld_table(table + idx0, streaming);
 	v1 = ld_table(table + idx1, streaming);
+	return 0u;
 }
 
 // Scatter-add two fp16x2 addends of a corner pair (red.global.add.noftz.f16x2 is what the reference's
