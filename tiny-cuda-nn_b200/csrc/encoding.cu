@@ -16,7 +16,6 @@
 #include "grid_kernels.h"
 #include "host_common.h"
 #include "json_mini.h"
-#include "misc_kernels.h"
 
 #include <memory>
 #include <vector>
@@ -25,30 +24,19 @@ namespace tcnnb {
 
 struct Encoding {
 	EncodingPlan plan;
-	DeviceBuffer<float> scratch;        // level scales; fp32 gradient accumulator when F == 1
-	DeviceBuffer<__half> replicas;      // private copies of the coarse levels' gradients (grid_kernels.h plan_grid_scatter)
 	float max_level = 1.0f;
 	std::string hyperparams_json;
 	uint32_t max_align = 2;             // strictest pointer alignment the kernels need for feature rows / parameters (bytes)
 };
 
 static void build_encoding(Encoding& e, uint32_t n_input_dims, const json::Value& cfg) {
-	int device = 0;
-	TCNNB_CUDA_CHECK(cudaGetDevice(&device));
-	cudaDeviceProp prop;
-	TCNNB_CUDA_CHECK(cudaGetDeviceProperties(&prop, device));
-	if (prop.major != 9) throw std::runtime_error("tcnn_b200 requires an sm_90-class GPU (H100); found compute capability " + std::to_string(prop.major) + "." + std::to_string(prop.minor));
-	e.scratch.resize(128);
-	build_encoding_plan(e.plan, n_input_dims, cfg, 0, e.scratch.ptr);
+	require_sm90();
+	build_encoding_plan(e.plan, n_input_dims, cfg, 0);
 	for (auto& g : e.plan.grids) {
 		e.max_align = std::max(e.max_align, 2 * g->cfg.n_features_per_level);
 		// feature rows are read / written with one vector access per level: every row has to start on that boundary
 		if (e.plan.width % g->cfg.n_features_per_level != 0) throw std::runtime_error("tcnn_b200: the total width of this Composite encoding must be a multiple of the grid's n_features_per_level");
 	}
-}
-
-static void check_n(uint32_t n) {
-	if (n == 0 || n % BATCH_GRANULARITY != 0) throw std::runtime_error("batch size " + std::to_string(n) + " must be a non-zero multiple of " + std::to_string(BATCH_GRANULARITY));
 }
 
 static void check_ptr(const void* p, const char* what, size_t align) {
@@ -84,19 +72,8 @@ uint32_t tcnnb_encoding_n_output_dims(const tcnnb_encoding* e) { return e->impl.
 // Level table of the (first) grid of the encoding; n_levels = 0 when there is none.
 int tcnnb_encoding_grid_levels(const tcnnb_encoding* e, uint32_t* n_levels, uint32_t* offsets, float* scales, uint32_t* resolutions) {
 	TCNNB_API_BEGIN
-	if (e->impl.plan.grids.empty()) {
-		if (n_levels) *n_levels = 0;
-		if (offsets) offsets[0] = 0;
-		return 0;
-	}
-	const GridConfig& g = e->impl.plan.grids.front()->cfg;
-	if (n_levels) *n_levels = g.n_levels;
-	for (uint32_t l = 0; l < g.n_levels; ++l) {
-		if (offsets) offsets[l] = g.offsets[l];
-		if (scales) scales[l] = g.scales[l];
-		if (resolutions) resolutions[l] = (uint32_t)ceilf(g.scales[l]) + 1;
-	}
-	if (offsets) offsets[g.n_levels] = g.offsets[g.n_levels];
+	const EncodingPlan& plan = e->impl.plan;
+	write_level_table(plan.grids.empty() ? nullptr : &plan.grids.front()->cfg, n_levels, offsets, scales, resolutions);
 	TCNNB_API_END
 }
 
@@ -111,11 +88,7 @@ int tcnnb_encoding_initialize_params(tcnnb_encoding* e, uint64_t seed, float* pa
 	if (e->impl.plan.n_params == 0) return 0;
 	if (!params_full_precision_dev) throw std::runtime_error("encoding: params_full_precision is null.");
 	HostPcg32 rng{seed};
-	for (auto& g : e->impl.plan.grids) {
-		TCNNB_CUDA_CHECK(launch_random_uniform(nullptr, rng.device(), g->cfg.n_params, params_full_precision_dev + g->param_offset, -1e-4f * scale, 1e-4f * scale));
-		++g_kernel_launches;
-		rng.advance(g->cfg.n_params);
-	}
+	init_plan_params(e->impl.plan, rng, params_full_precision_dev, scale);
 	TCNNB_CUDA_CHECK(cudaDeviceSynchronize());
 	TCNNB_API_END
 }
@@ -123,23 +96,11 @@ int tcnnb_encoding_initialize_params(tcnnb_encoding* e, uint64_t seed, float* pa
 int tcnnb_encoding_forward(tcnnb_encoding* e, tcnnb_stream stream, uint32_t n_elements, const float* input_dev, void* output_dev, const void* params_dev) {
 	TCNNB_API_BEGIN
 	Encoding& enc = e->impl;
-	const EncodingPlan& plan = enc.plan;
-	check_n(n_elements);
+	check_batch(n_elements);
 	check_ptr(input_dev, "input", 4);
 	check_ptr(output_dev, "output", enc.max_align);
-	if (plan.n_params) check_ptr(params_dev, "params", enc.max_align);
-	cudaStream_t s = (cudaStream_t)stream;
-	if (plan.has_plain_features()) {
-		TCNNB_CUDA_CHECK(launch_feature_forward(s, plan.segs, n_elements, input_dev, plan.n_in, (__half*)output_dev, plan.width));
-		++g_kernel_launches;
-	}
-	for (auto& g : plan.grids) {
-		const FeatureSegment& sg = plan.segs.s[g->segment];
-		GridKernelArgs a = plan_grid_args(*g, n_elements, input_dev + sg.in_begin, plan.n_in, plan.width, enc.max_level);
-		a.pad_cols = sg.n_pad;
-		TCNNB_CUDA_CHECK(launch_grid_forward(s, a, (const __half*)params_dev + g->param_offset, (__half*)output_dev + sg.out_begin));
-		++g_kernel_launches;
-	}
+	if (enc.plan.n_params) check_ptr(params_dev, "params", enc.max_align);
+	plan_forward(enc.plan, (cudaStream_t)stream, n_elements, input_dev, (const __half*)params_dev, (__half*)output_dev, enc.plan.width, enc.max_level);
 	TCNNB_API_END
 }
 
@@ -147,55 +108,16 @@ int tcnnb_encoding_backward(tcnnb_encoding* e, tcnnb_stream stream, uint32_t n_e
                             const void* params_dev) {
 	TCNNB_API_BEGIN
 	Encoding& enc = e->impl;
-	const EncodingPlan& plan = enc.plan;
-	check_n(n_elements);
+	EncodingPlan& plan = enc.plan;
+	check_batch(n_elements);
 	check_ptr(input_dev, "input", 4);
 	check_ptr(dL_doutput_dev, "dL_doutput", enc.max_align);
+	if (dL_dparams_dev && plan.n_params) check_ptr(dL_dparams_dev, "dL_dparams", enc.max_align);
+	if (dL_dinput_dev && !plan.grids.empty()) check_ptr(params_dev, "params", enc.max_align);
 	cudaStream_t s = (cudaStream_t)stream;
 	const __half* dy = (const __half*)dL_doutput_dev;
-	if (dL_dparams_dev && plan.n_params) {  // GradientMode::Overwrite (src/cpp_api.cu:115)
-		check_ptr(dL_dparams_dev, "dL_dparams", enc.max_align);
-		TCNNB_CUDA_CHECK(cudaMemsetAsync(dL_dparams_dev, 0, sizeof(__half) * plan.n_params, s));
-		for (auto& g : plan.grids) {
-			const FeatureSegment& sg = plan.segs.s[g->segment];
-			const uint32_t F = g->cfg.n_features_per_level;
-			GridKernelArgs a = plan_grid_args(*g, n_elements, input_dev + sg.in_begin, plan.n_in, plan.width, enc.max_level);
-			if (enc.max_level >= 1.0f) {  // contended coarse levels scatter into private copies
-				const GridScatterPlan sp = plan_grid_scatter(g->levels.data(), g->cfg.n_levels, F, g->cfg.n_pos_dims, n_elements);
-				if (sp.n_replicas > 1) {
-					if (enc.replicas.n < sp.scratch_halfs) {
-						enc.replicas.resize(sp.scratch_halfs);
-						enc.replicas.zero(s);
-					}
-					a.replica_scratch = enc.replicas.ptr;
-					a.n_replicas = sp.n_replicas;
-					a.replica_entries = sp.replica_entries;
-				}
-			}
-			float* tmp = nullptr;
-			if (F == 1) {
-				enc.scratch.resize(std::max<size_t>(enc.scratch.n, g->cfg.n_params));
-				tmp = enc.scratch.ptr;
-				TCNNB_CUDA_CHECK(cudaMemsetAsync(tmp, 0, sizeof(float) * g->cfg.n_params, s));
-			}
-			TCNNB_CUDA_CHECK(launch_grid_backward(s, a, dy + sg.out_begin, (__half*)dL_dparams_dev + g->param_offset, tmp, g->cfg.n_params));
-			g_kernel_launches += F == 1 ? 2 : 1;
-		}
-	}
-	if (dL_dinput_dev) {
-		if (plan.composite) TCNNB_CUDA_CHECK(cudaMemsetAsync(dL_dinput_dev, 0, sizeof(float) * (size_t)n_elements * plan.n_in, s));
-		if (plan.has_plain_features()) {
-			TCNNB_CUDA_CHECK(launch_feature_input_gradient(s, plan.segs, n_elements, input_dev, plan.n_in, dy, plan.width, dL_dinput_dev));
-			++g_kernel_launches;
-		}
-		for (auto& g : plan.grids) {
-			const FeatureSegment& sg = plan.segs.s[g->segment];
-			check_ptr(params_dev, "params", enc.max_align);
-			const GridKernelArgs a = plan_grid_args(*g, n_elements, input_dev + sg.in_begin, plan.n_in, plan.width, enc.max_level);
-			TCNNB_CUDA_CHECK(launch_grid_input_gradient(s, a, (const __half*)params_dev + g->param_offset, dy + sg.out_begin, dL_dinput_dev + sg.in_begin));
-			++g_kernel_launches;
-		}
-	}
+	if (dL_dparams_dev) plan_param_gradients(plan, s, n_elements, input_dev, dy, plan.width, (__half*)dL_dparams_dev, enc.max_level);  // GradientMode::Overwrite (src/cpp_api.cu:115)
+	if (dL_dinput_dev) plan_input_gradient(plan, s, n_elements, input_dev, (const __half*)params_dev, dy, plan.width, dL_dinput_dev, enc.max_level);
 	TCNNB_API_END
 }
 

@@ -1,6 +1,6 @@
 // encoding_plan.h -- an encoding configuration (src/encoding.cu:60-150) resolved into a table of segments: which input dimensions each
 // (nested) encoding reads, which output columns it writes, how it is padded, where its parameters live. Shared by the general path of
-// the model (model.cu) and the encoding tier (encoding.cu).
+// the model (model.cu) and the encoding tier (encoding.cu), which both run it with the plan operations below (encoding_plan.cu).
 //
 // Composite (encodings/composite.h:135-215): "nested" array, each entry with "n_dims_to_encode" (one entry may leave it out and takes
 // the remaining dimensions); outputs are concatenated; every nested encoding but the last is padded so that the NEXT one starts at a
@@ -35,6 +35,9 @@ struct EncodingPlan {
 	bool composite = false;
 	FeatureSegments segs{};
 	std::vector<std::unique_ptr<Grid>> grids;
+	// scratch of the table-gradient scatter (plan_param_gradients), grown on demand
+	DeviceBuffer<float> grad_fp32;     // n_features_per_level == 1: fp32 scatter target (grid.h:858-894)
+	DeviceBuffer<__half> replicas;     // private copies of the coarse levels' gradients (grid_kernels.h plan_grid_scatter); zero between uses
 	bool has_plain_features() const {
 		for (uint32_t i = 0; i < segs.n; ++i) if (segs.s[i].type != FEAT_GRID) return true;
 		return false;
@@ -104,8 +107,7 @@ inline uint32_t required_alignment(const EncodingPlan& plan, uint32_t seg) { ret
 }  // namespace plan_detail
 
 // `alignment`: what the consumer needs the padded width to be a multiple of (16 in front of a network, 1 for cpp::create_encoding).
-// `scales_scratch_dev`: >= 128 floats of device memory (per-level grid scales are evaluated on the device).
-inline void build_encoding_plan(EncodingPlan& plan, uint32_t n_in, const json::Value& cfg, uint32_t alignment, float* scales_scratch_dev) {
+inline void build_encoding_plan(EncodingPlan& plan, uint32_t n_in, const json::Value& cfg, uint32_t alignment) {
 	using namespace plan_detail;
 	plan.n_in = n_in;
 	const std::string lower = to_lower(cfg.value("otype", "OneBlob"));
@@ -160,7 +162,7 @@ inline void build_encoding_plan(EncodingPlan& plan, uint32_t n_in, const json::V
 		g->param_offset = param_offset;
 		param_offset += g->cfg.n_params;
 		g->cfg.padded_width = g->cfg.n_levels * g->cfg.n_features_per_level;
-		evaluate_level_scales(g->cfg, scales_scratch_dev);
+		evaluate_level_scales(g->cfg);
 		g->levels.resize(g->cfg.n_levels);
 		for (uint32_t l = 0; l < g->cfg.n_levels; ++l) g->levels[l] = make_level_info(g->cfg, l);
 		g->levels_dev.resize(g->levels.size());
@@ -185,5 +187,23 @@ inline GridKernelArgs plan_grid_args(const EncodingPlan::Grid& g, uint32_t n, co
 	a.row_stride = row_stride;
 	return a;
 }
+
+// ---- running a plan (encoding_plan.cu). Positions are rows [n][plan.n_in] fp32; encoded features and dL/d(encoded) are fp16 rows
+// [n][row_stride] whose first plan.width columns belong to the plan; `params` / `dL_dparams` hold the plan's own n_params entries.
+// `max_level`: fraction of the grid levels that is active (GridEncoding::set_max_level); 1 = all. Each adds the kernels it
+// launches to g_kernel_launches.
+
+// encoded = features of the n samples (padding columns included)
+void plan_forward(const EncodingPlan& plan, cudaStream_t stream, uint32_t n, const float* x, const __half* params, __half* encoded, uint32_t row_stride, float max_level);
+// dL_dparams (OVERWRITTEN, GradientMode::Overwrite) = the grids' table gradients. Contended coarse levels scatter into private
+// copies when max_level >= 1.
+void plan_param_gradients(EncodingPlan& plan, cudaStream_t stream, uint32_t n, const float* x, const __half* dL_dencoded, uint32_t row_stride, __half* dL_dparams,
+                          float max_level);
+// dL_dx [n][plan.n_in] fp32 (OVERWRITTEN) = dL/d(encoded) contracted with d(encoded)/d(position)
+void plan_input_gradient(const EncodingPlan& plan, cudaStream_t stream, uint32_t n, const float* x, const __half* params, const __half* dL_dencoded, uint32_t row_stride,
+                         float* dL_dx, float max_level);
+// Grid tables U(-1e-4, 1e-4) * scale from `rng`, nested grids one after the other (grid.h:1076-1079, composite.h initialize_params).
+// `dst`: DEVICE fp32 array of plan.n_params elements.
+void init_plan_params(const EncodingPlan& plan, HostPcg32& rng, float* dst, float scale);
 
 }  // namespace tcnnb

@@ -116,12 +116,27 @@ inline GridConfig parse_grid(uint32_t n_dims_to_encode, const json::Value& e) {
 
 
 // Per-level scales evaluated on the DEVICE like the reference's kernels (common_device.h:886-891; fast-math ex2.approx + fma), so
-// that cell selection matches them bit for bit. `scratch_dev`: at least 128 floats of device memory.
-inline void evaluate_level_scales(GridConfig& g, float* scratch_dev) {
+// that cell selection matches them bit for bit.
+inline void evaluate_level_scales(GridConfig& g) {
+	DeviceBuffer<float> scales_dev;
+	scales_dev.resize(g.n_levels);
 	g.scales.resize(g.n_levels);
-	TCNNB_CUDA_CHECK(launch_level_scales(nullptr, g.n_levels, std::log2(g.per_level_scale), g.base_resolution, scratch_dev));
+	TCNNB_CUDA_CHECK(launch_level_scales(nullptr, g.n_levels, std::log2(g.per_level_scale), g.base_resolution, scales_dev.ptr));
 	++g_kernel_launches;
-	TCNNB_CUDA_CHECK(cudaMemcpy(g.scales.data(), scratch_dev, sizeof(float) * g.n_levels, cudaMemcpyDeviceToHost));
+	TCNNB_CUDA_CHECK(cudaMemcpy(g.scales.data(), scales_dev.ptr, sizeof(float) * g.n_levels, cudaMemcpyDeviceToHost));
+}
+
+// The level table as the C ABI exports it (ParamsOffsetTable, multi_level_interface.h:84-88): n_levels, n_levels + 1 offsets,
+// and per level the scale and resolution. `g` == nullptr: no grid (n_levels = 0, offsets = {0}). Every output is optional.
+inline void write_level_table(const GridConfig* g, uint32_t* n_levels, uint32_t* offsets, float* scales, uint32_t* resolutions) {
+	const uint32_t n = g ? g->n_levels : 0;
+	if (n_levels) *n_levels = n;
+	for (uint32_t l = 0; l < n; ++l) {
+		if (offsets) offsets[l] = g->offsets[l];
+		if (scales) scales[l] = g->scales[l];
+		if (resolutions) resolutions[l] = (uint32_t)ceilf(g->scales[l]) + 1;
+	}
+	if (offsets) offsets[n] = g ? g->offsets[n] : 0;
 }
 
 // LevelInfo of level l (needs g.scales).

@@ -1,5 +1,6 @@
-// host_common.h -- host-side helpers shared by the C-ABI translation units (model.cu: trainer / module tiers; network.cu: the
-// stand-alone network tier): error plumbing, device buffers, the host pcg32, name tables.
+// host_common.h -- host-side helpers shared by the C-ABI translation units (model.cu: trainer / module tiers; network.cu and
+// encoding.cu: the stand-alone network and encoding tiers): error plumbing, device buffers, the device and batch checks, the host
+// pcg32, name tables.
 #pragma once
 #include "common.cuh"
 
@@ -92,6 +93,28 @@ struct DeviceBuffer {
 		if (n) TCNNB_CUDA_CHECK(cudaMemsetAsync(ptr, 0, n * sizeof(T), stream));
 	}
 };
+
+template <typename T>
+inline void grow(DeviceBuffer<T>& b, size_t n) {
+	if (b.n < n) b.resize(n);
+}
+
+// The current device must be an sm_90-class GPU (the kernels are built for sm_90a only). Returns its SM count.
+inline int require_sm90() {
+	int device = 0;
+	TCNNB_CUDA_CHECK(cudaGetDevice(&device));
+	cudaDeviceProp prop;
+	TCNNB_CUDA_CHECK(cudaGetDeviceProperties(&prop, device));
+	if (prop.major != 9) throw std::runtime_error("tcnn_b200 requires an sm_90-class GPU (H100); found compute capability " + std::to_string(prop.major) + "." + std::to_string(prop.minor));
+	return prop.multiProcessorCount;
+}
+
+inline void check_batch(uint32_t batch) {
+	if (batch == 0 || batch % BATCH_GRANULARITY != 0) {
+		// object.h:169: CHECK_THROW(input.n() % BATCH_SIZE_GRANULARITY == 0)
+		throw std::runtime_error("batch size " + std::to_string(batch) + " must be a non-zero multiple of " + std::to_string(BATCH_GRANULARITY));
+	}
+}
 
 
 inline uint32_t parse_activation(const std::string& name) {

@@ -21,6 +21,7 @@
 #include "json_mini.h"
 #include "misc_kernels.h"
 #include "mlp_fused.h"
+#include "network_config.h"
 
 #include <dlfcn.h>
 #include <nccl.h>  // types and prototypes only: libnccl is resolved at run time (dlopen), single-GPU users never need it
@@ -42,18 +43,6 @@ namespace tcnnb {
 
 std::atomic<uint64_t> g_kernel_launches{0};
 thread_local std::string g_last_error;
-
-struct MlpConfig {
-	std::string otype = "FullyFusedMLP";
-	uint32_t in_width = 0;
-	uint32_t width = 128;
-	uint32_t n_hidden_layers = 5;
-	uint32_t out_width = 0;
-	uint32_t padded_out_width = 0;
-	uint32_t activation = ACT_RELU;
-	uint32_t output_activation = ACT_NONE;
-	uint32_t n_params = 0;
-};
 
 // ------------------------------------------------------------------------------------------------ NCCL (data parallel)
 // libnccl.so.2 is looked up when the first data-parallel call is made. In a PyTorch process this resolves to the copy
@@ -141,7 +130,6 @@ struct Model {
 	DeviceBuffer<float> ema_tmp;
 	const __half* inference_params() const { return ema.enabled ? ema_fp16.ptr : params_fp16; }
 	float loss_scale = 128.0f;  // default_loss_scale<__half>() (common.h:243)
-	int device = 0;
 	int n_sms = 132;
 
 	size_t n_params = 0;
@@ -157,10 +145,8 @@ struct Model {
 	DeviceBuffer<float> dw_accum;   // fp32 MLP weight-gradient accumulator
 	DeviceBuffer<float> scalars;    // [0] = loss sum
 	DeviceBuffer<long long> dbg_clock;  // TCNNB_CLOCKS=<file> in ablation builds: phase stamps of the last ws launch
-	DeviceBuffer<float> level_scales_dev;
 	bool enc_identity = false;              // "Identity" encoding instead of a grid (no encoding parameters)
 	float identity_scale = 1.0f, identity_offset = 0.0f;
-	DeviceBuffer<LevelInfo> levels_dev;     // per-level descriptors for the stand-alone grid kernels (module tier: dL/d(input))
 	DeviceBuffer<__half> denc_scratch;      // module tier: dL/d(encoded) rows [n][64] handed from the fused kernel to the input-gradient kernel
 	DeviceBuffer<__half> grads_scratch;     // module tier: gradient array when the caller wants dL/d(input) only
 	bool mlp_grads_in_accum = false;
@@ -171,12 +157,9 @@ struct Model {
 	bool force_general = false;  // tcnnb_debug_set("general", 1): run the general path although the fused kernel covers the configuration
 	bool use_general() const { return general || force_general; }
 	bool plan_only = false;      // an encoding other than one grid / Identity (Composite, Frequency, OneBlob, ...): no fused kernel at all
-	EncodingPlan plan;           // segment table of the encoding (general path)
+	EncodingPlan plan;           // segment table of the encoding (general path; module tier: dL/d(input))
 	std::string general_reason;  // which limit of the fused kernel sent this configuration here (hyperparams / diagnostics)
 	DeviceBuffer<__half> g_enc, g_hidden, g_out, g_dy, g_grad_hidden, g_denc, g_dy_act;
-	DeviceBuffer<float> g_grid_tmp;  // n_features_per_level == 1: fp32 scatter target (grid.h:858-894)
-	DeviceBuffer<__half> g_replicas; // private copies of the coarse levels' gradients (grid_kernels.h plan_grid_scatter)
-	int grid_replicas_override = -1; // tcnnb_debug_set("grid_replicas", n): experiments (0 / 1 = off)
 
 	// spatial binning scratch (binning.cu): sorted copies of the batch + permutation
 	bool binning = true;  // tcnnb_debug_set("binning", 0) (tests: binned and unbinned steps must touch the same entries)
@@ -258,43 +241,26 @@ struct Model {
 // initialize_params(rnd, params_full_precision, scale) of NetworkWithInputEncoding (network_with_input_encoding.h:124-130):
 // network weights first, then the grid table, one pcg32 stream. `dst` is a DEVICE fp32 array of n_params elements.
 static void init_params(Model& m, HostPcg32& rng, float* dst, float scale) {
-	const MlpConfig& mlp = m.mlp;
-	// MLP: xavier uniform on the host, sequential draws (fully_fused_mlp.cu:868-892, gpu_matrix.h:292-306)
-	{
-		std::vector<float> w(mlp.n_params);
-		std::vector<std::pair<uint32_t, uint32_t>> mats;
-		mats.emplace_back(mlp.width, mlp.in_width);
-		for (uint32_t i = 0; i + 1 < mlp.n_hidden_layers; ++i) mats.emplace_back(mlp.width, mlp.width);
-		mats.emplace_back(mlp.padded_out_width, mlp.width);
-		size_t pos = 0;
-		for (auto& rc : mats) {
-			const float bound = scale * std::sqrt(6.0f / (float)(rc.second + rc.first));
-			for (size_t i = 0; i < (size_t)rc.first * rc.second; ++i) w[pos++] = rng.next_float() * 2.0f * bound - bound;
-		}
-		TCNNB_CUDA_CHECK(cudaMemcpy(dst, w.data(), sizeof(float) * w.size(), cudaMemcpyHostToDevice));
-	}
-	// grid: U(-1e-4, 1e-4) * scale generated on the device with the jump-ahead pattern (grid.h:1076-1079, random.h:56-69)
-	if (m.plan_only) {  // nested encodings draw one after the other from the same stream (composite.h initialize_params)
-		for (auto& g : m.plan.grids) {
-			TCNNB_CUDA_CHECK(launch_random_uniform(nullptr, rng.device(), g->cfg.n_params, dst + mlp.n_params + g->param_offset, -1e-4f * scale, 1e-4f * scale));
-			++g_kernel_launches;
-			rng.advance(g->cfg.n_params);
-		}
-	} else if (m.grid.n_params) {
-		TCNNB_CUDA_CHECK(launch_random_uniform(nullptr, rng.device(), m.grid.n_params, dst + mlp.n_params, -1e-4f * scale, 1e-4f * scale));
-		++g_kernel_launches;
-		rng.advance(m.grid.n_params);
-	}
+	init_mlp_params(m.mlp, rng, dst, scale);
+	init_plan_params(m.plan, rng, dst + m.mlp.n_params, scale);  // nested encodings draw one after the other from the same stream
+}
+
+// Whether the stand-alone network kernels cover this network (they have their own limits, e.g. dL/d(encoded) wider than the layers):
+// nullptr, else the reason they do not.
+static const char* general_path_unsupported(const Model& m) {
+	MlpBackwardArgs probe{};
+	probe.width = m.mlp.width;
+	probe.in_width = m.mlp.in_width;
+	probe.out_width = m.mlp.padded_out_width;
+	probe.n_hidden_layers = m.mlp.n_hidden_layers;
+	probe.batch_size = 256;
+	probe.dL_dinput = m.grid.n_params == 0 ? nullptr : (__half*)16;  // the encoding's backward pass needs dL/d(encoded)
+	const char* why_not = nullptr;
+	return mlp_backward_supported(probe, &why_not) ? nullptr : why_not;
 }
 
 static void build_model(Model& m, uint32_t n_in, uint32_t n_out, const json::Value& cfg, uint32_t seed, bool module_only = false) {
-	TCNNB_CUDA_CHECK(cudaGetDevice(&m.device));
-	cudaDeviceProp prop;
-	TCNNB_CUDA_CHECK(cudaGetDeviceProperties(&prop, m.device));
-	if (prop.major != 9) {
-		throw std::runtime_error("tcnn_b200 requires an sm_90-class GPU (H100); found compute capability " + std::to_string(prop.major) + "." + std::to_string(prop.minor));
-	}
-	m.n_sms = prop.multiProcessorCount;
+	m.n_sms = require_sm90();
 #ifdef TCNNB_ENABLE_ABLATION  // profiling builds only (make ABLATION=1); the production library reads no environment switches
 	if (const char* e = std::getenv("TCNNB_ABLATE")) m.ablate = (uint32_t)std::atoi(e);
 	if (std::getenv("TCNNB_CLOCKS")) {
@@ -368,22 +334,7 @@ static void build_model(Model& m, uint32_t n_in, uint32_t n_out, const json::Val
 	a.optimize_non_matrix_params = opt.value("optimize_non_matrix_params", true);
 	a.skip_zero_grad_non_matrix_params = opt.value("skip_zero_grad_non_matrix_params", true);
 
-	// ---- network (src/network.cu:51-141) and encoding alignment (network_with_input_encoding.h:47)
-	const json::Value& net = cfg.sub("network");
-	MlpConfig& mlp = m.mlp;
-	mlp.otype = net.value("otype", "MLP");
-	const bool fully_fused = ieq(mlp.otype, "FullyFusedMLP") || ieq(mlp.otype, "MegakernelMLP");
-	const bool cutlass = ieq(mlp.otype, "MLP") || ieq(mlp.otype, "CutlassMLP");
-	if (!fully_fused && !cutlass) throw std::runtime_error("Invalid network type: " + mlp.otype);
-	mlp.width = (uint32_t)net.value("n_neurons", 128.0);
-	mlp.n_hidden_layers = (uint32_t)net.value("n_hidden_layers", 5.0);
-	mlp.activation = parse_activation(net.value("activation", "ReLU"));
-	mlp.output_activation = parse_activation(net.value("output_activation", "None"));
-	if (fully_fused && !(mlp.width == 16 || mlp.width == 32 || mlp.width == 64 || mlp.width == 128)) {
-		throw std::runtime_error("FullyFusedMLP only supports 16, 32, 64, and 128 neurons, but got " + std::to_string(mlp.width) + ". Use CutlassMLP instead if this is a requirement.");
-	}
-	if (mlp.n_hidden_layers < 1) throw std::runtime_error("FullyFusedMLP requires at least 1 hidden layer (3 layers in total).");
-
+	// ---- encoding, padded to the network's alignment (network_with_input_encoding.h:47)
 	const uint32_t alignment = 16;  // FullyFusedMLP / CutlassMLP REQUIRED_ALIGNMENT (src/network.cu:79-98)
 	const json::Value& enc_cfg = cfg.sub("encoding");
 	if (ieq(enc_cfg.value("otype", "OneBlob"), "Identity")) {
@@ -407,8 +358,7 @@ static void build_model(Model& m, uint32_t n_in, uint32_t n_out, const json::Val
 		// Composite / Frequency / TriangleWave / OneBlob / SphericalHarmonics (src/encoding.cu:60-120): stand-alone encoding kernels in
 		// front of the stand-alone network kernels. `grid` only carries the totals the rest of the model needs.
 		m.plan_only = true;
-		m.level_scales_dev.resize(128);
-		build_encoding_plan(m.plan, n_in, enc_cfg, alignment, m.level_scales_dev.ptr);
+		build_encoding_plan(m.plan, n_in, enc_cfg, alignment);
 		m.grid = GridConfig{};
 		m.grid.otype = enc_cfg.value("otype", "OneBlob");
 		m.grid.n_pos_dims = n_in;
@@ -418,17 +368,12 @@ static void build_model(Model& m, uint32_t n_in, uint32_t n_out, const json::Val
 		m.grid.padded_width = m.plan.width;
 	}
 
-	mlp.in_width = m.grid.padded_width;
-	mlp.out_width = n_out;
-	mlp.padded_out_width = next_multiple(n_out, 16u);
-	mlp.n_params = mlp.width * mlp.in_width + (mlp.n_hidden_layers - 1) * mlp.width * mlp.width + mlp.padded_out_width * mlp.width;
+	// ---- network (src/network.cu:51-141)
+	MlpConfig& mlp = m.mlp;
+	mlp = parse_network(cfg.sub("network"), m.grid.padded_width, n_out);
 
 	// ---- which kernels run this configuration. The fused kernel (fused_ws.cu) covers the benchmarked family; everything else the
 	// stand-alone kernels cover takes the general path; the rest fails loudly (no fallback to anything that is not a kernel of this library).
-	// FullyFusedMLP's activation set (fully_fused_mlp.cu:689-699): Sine and SiLU need stored pre-activations and are rejected there too.
-	for (uint32_t act : {mlp.activation, mlp.output_activation}) {
-		if (act == ACT_SINE || act == ACT_SILU) throw std::runtime_error("Unsupported activation.");
-	}
 	if (m.grid.stochastic_interpolation) throw std::runtime_error("tcnn_b200: stochastic_interpolation is not built");
 	{
 		const char* why = nullptr;
@@ -444,15 +389,7 @@ static void build_model(Model& m, uint32_t n_in, uint32_t n_out, const json::Val
 		if (why) {
 			m.general = true;
 			m.general_reason = why;
-			MlpBackwardArgs probe{};
-			probe.width = mlp.width;
-			probe.in_width = mlp.in_width;
-			probe.out_width = mlp.padded_out_width;
-			probe.n_hidden_layers = mlp.n_hidden_layers;
-			probe.batch_size = 256;
-			probe.dL_dinput = m.grid.n_params == 0 ? nullptr : (__half*)16;  // the encoding's backward pass needs dL/d(encoded)
-			const char* why_not = nullptr;
-			if (!mlp_backward_supported(probe, &why_not)) throw std::runtime_error(std::string(why_not) + " (general path of tcnn_b200; the fused kernel does not cover this configuration: " + why + ")");
+			if (const char* why_not = general_path_unsupported(m)) throw std::runtime_error(std::string(why_not) + " (general path of tcnn_b200; the fused kernel does not cover this configuration: " + why + ")");
 			if (!m.enc_identity && !m.plan_only) {
 				const uint32_t F = m.grid.n_features_per_level, D = m.grid.n_pos_dims;
 				if (!(F == 1 || F == 2 || F == 4 || F == 8)) throw std::runtime_error("GridEncoding: n_features_per_level must be 1, 2, 4, or 8.");
@@ -462,11 +399,11 @@ static void build_model(Model& m, uint32_t n_in, uint32_t n_out, const json::Val
 	}
 
 	// ---- per-level scales, evaluated on the device like the reference's kernels (common_device.h:886-891)
-	m.level_scales_dev.resize(128);
-	if (!m.enc_identity && !m.plan_only) evaluate_level_scales(m.grid, m.level_scales_dev.ptr);
+	if (!m.enc_identity && !m.plan_only) evaluate_level_scales(m.grid);
 	// one grid / Identity: the segment table of the general path is built for every configuration, so that the general path can run what
-	// the fused kernel also covers (tests: both paths must agree; tcnnb_debug_set("general", 1))
-	if (!m.plan_only) build_encoding_plan(m.plan, n_in, enc_cfg, alignment, m.level_scales_dev.ptr);
+	// the fused kernel also covers (tests: both paths must agree; tcnnb_debug_set("general", 1)) and the module tier's dL/d(input) runs
+	// through it
+	if (!m.plan_only) build_encoding_plan(m.plan, n_in, enc_cfg, alignment);
 
 	// ---- parameter buffers (trainer.h:69-87,489-503)
 	m.n_params = (size_t)mlp.n_params + m.grid.n_params;
@@ -519,13 +456,6 @@ static void build_model(Model& m, uint32_t n_in, uint32_t n_out, const json::Val
 		TCNNB_CUDA_CHECK(cudaEventCreateWithFlags(&sl.ev_in, cudaEventDisableTiming));
 		TCNNB_CUDA_CHECK(cudaEventCreateWithFlags(&sl.ev_target, cudaEventDisableTiming));
 		TCNNB_CUDA_CHECK(cudaEventCreateWithFlags(&sl.ev_done, cudaEventDisableTiming));
-	}
-}
-
-static void check_batch(uint32_t batch) {
-	if (batch == 0 || batch % BATCH_GRANULARITY != 0) {
-		// object.h:169: CHECK_THROW(input.n() % BATCH_SIZE_GRANULARITY == 0)
-		throw std::runtime_error("batch size " + std::to_string(batch) + " must be a non-zero multiple of " + std::to_string(BATCH_GRANULARITY));
 	}
 }
 
@@ -618,52 +548,11 @@ static void optimizer_step(Model& m, cudaStream_t stream, uint32_t n_ranges = 0,
 	}
 }
 
-static void ensure_levels_dev(Model& m, cudaStream_t stream) {
-	if (m.levels_dev.n == 0 && m.grid.n_levels) {
-		std::vector<LevelInfo> levels(m.grid.n_levels);
-		for (uint32_t l = 0; l < m.grid.n_levels; ++l) levels[l] = make_level_info(m.grid, l);
-		m.levels_dev.resize(levels.size());
-		TCNNB_CUDA_CHECK(cudaMemcpyAsync(m.levels_dev.ptr, levels.data(), sizeof(LevelInfo) * levels.size(), cudaMemcpyHostToDevice, stream));
-		TCNNB_CUDA_CHECK(cudaStreamSynchronize(stream));  // `levels` is a pageable temporary
-	}
-}
-
-static GridKernelArgs grid_kernel_args(Model& m, uint32_t n, const float* x, uint32_t row_stride) {
-	GridKernelArgs a{};
-	a.n_pos_dims = m.grid.n_pos_dims;
-	a.n_features_per_level = m.grid.n_features_per_level;
-	a.n_levels = m.grid.n_levels;
-	a.interpolation = m.grid.interpolation;
-	a.max_level = 1.0f;
-	a.levels_dev = m.levels_dev.ptr;
-	a.n_elements = n;
-	a.positions = x;
-	a.pos_stride = m.grid.n_pos_dims;
-	a.row_stride = row_stride;
-	a.pad_cols = row_stride - m.grid.n_levels * m.grid.n_features_per_level;
-	return a;
-}
-
-template <typename T>
-static void grow(DeviceBuffer<T>& b, size_t n) {
-	if (b.n < n) b.resize(n);
-}
-
 // ---- general path: encoding kernel -> stand-alone network kernel (mlp_fused.cu), activations optionally kept for the backward pass
 static void general_forward(Model& m, cudaStream_t stream, uint32_t batch, const float* x, const __half* params, __half* out_fp16, float* out_fp32, bool keep_hidden) {
 	const MlpConfig& mlp = m.mlp;
 	grow(m.g_enc, (size_t)batch * mlp.in_width);
-	if (m.plan.has_plain_features()) {
-		TCNNB_CUDA_CHECK(launch_feature_forward(stream, m.plan.segs, batch, x, m.n_in, m.g_enc.ptr, mlp.in_width));
-		++g_kernel_launches;
-	}
-	for (auto& g : m.plan.grids) {
-		const FeatureSegment& sg = m.plan.segs.s[g->segment];
-		GridKernelArgs ga = plan_grid_args(*g, batch, x + sg.in_begin, m.n_in, mlp.in_width);
-		ga.pad_cols = sg.n_pad;
-		TCNNB_CUDA_CHECK(launch_grid_forward(stream, ga, params + mlp.n_params + g->param_offset, m.g_enc.ptr + sg.out_begin));
-		++g_kernel_launches;
-	}
+	plan_forward(m.plan, stream, batch, x, params + mlp.n_params, m.g_enc.ptr, mlp.in_width, 1.0f);
 	MlpForwardParams p{};
 	p.width = mlp.width;
 	p.in_width = mlp.in_width;
@@ -694,9 +583,6 @@ static void general_backward_pass(Model& m, cudaStream_t stream, uint32_t batch,
                                   const __half* ext_dL_doutput, float* dL_dinput, bool want_param_grads) {
 	const MlpConfig& mlp = m.mlp;
 	const bool grid_params = m.grid.n_params != 0 && want_param_grads;
-	if (grid_params) {
-		TCNNB_CUDA_CHECK(cudaMemsetAsync(grads + mlp.n_params, 0, sizeof(__half) * m.grid.n_params, stream));  // GradientMode::Overwrite (grid.h:865-867)
-	}
 	if (!ext_dL_doutput) TCNNB_CUDA_CHECK(cudaMemsetAsync(m.scalars.ptr, 0, sizeof(float), stream));
 	if (m.mlp_grads_in_accum) {
 		TCNNB_CUDA_CHECK(cudaMemsetAsync(m.dw_accum.ptr, 0, sizeof(float) * mlp.n_params, stream));
@@ -752,47 +638,8 @@ static void general_backward_pass(Model& m, cudaStream_t stream, uint32_t batch,
 	TCNNB_CUDA_CHECK(launch_mlp_backward(a, (uint32_t)m.n_sms, stream, &launches));
 	g_kernel_launches += launches;
 	if (want_param_grads) m.mlp_grads_in_accum = true;
-	if (grid_params) {
-		for (auto& g : m.plan.grids) {
-			const FeatureSegment& sg = m.plan.segs.s[g->segment];
-			float* tmp = nullptr;
-			if (g->cfg.n_features_per_level == 1) {
-				grow(m.g_grid_tmp, g->cfg.n_params);
-				TCNNB_CUDA_CHECK(cudaMemsetAsync(m.g_grid_tmp.ptr, 0, sizeof(float) * g->cfg.n_params, stream));
-				tmp = m.g_grid_tmp.ptr;
-			}
-			GridKernelArgs ga = plan_grid_args(*g, batch, x + sg.in_begin, m.n_in, mlp.in_width);
-			GridScatterPlan sp = plan_grid_scatter(g->levels.data(), g->cfg.n_levels, g->cfg.n_features_per_level, g->cfg.n_pos_dims, batch);
-			if (m.grid_replicas_override >= 0 && sp.replica_entries) {
-				sp.n_replicas = (uint32_t)m.grid_replicas_override;
-				sp.scratch_halfs = (size_t)sp.n_replicas * sp.replica_entries * g->cfg.n_features_per_level;
-			}
-			if (sp.n_replicas > 1) {
-				if (m.g_replicas.n < sp.scratch_halfs) {
-					m.g_replicas.resize(sp.scratch_halfs);
-					m.g_replicas.zero(stream);  // the reduce kernel leaves it zero
-				}
-				ga.replica_scratch = m.g_replicas.ptr;
-				ga.n_replicas = sp.n_replicas;
-				ga.replica_entries = sp.replica_entries;
-			}
-			TCNNB_CUDA_CHECK(launch_grid_backward(stream, ga, m.g_denc.ptr + sg.out_begin, grads + mlp.n_params + g->param_offset, tmp, g->cfg.n_params));
-			++g_kernel_launches;
-		}
-	}
-	if (dL_dinput) {
-		if (m.plan.composite) TCNNB_CUDA_CHECK(cudaMemsetAsync(dL_dinput, 0, sizeof(float) * (size_t)batch * m.n_in, stream));  // dimensions no nested encoding reads
-		if (m.plan.has_plain_features()) {
-			TCNNB_CUDA_CHECK(launch_feature_input_gradient(stream, m.plan.segs, batch, x, m.n_in, m.g_denc.ptr, mlp.in_width, dL_dinput));
-			++g_kernel_launches;
-		}
-		for (auto& g : m.plan.grids) {
-			const FeatureSegment& sg = m.plan.segs.s[g->segment];
-			const GridKernelArgs ga = plan_grid_args(*g, batch, x + sg.in_begin, m.n_in, mlp.in_width);
-			TCNNB_CUDA_CHECK(launch_grid_input_gradient(stream, ga, params + mlp.n_params + g->param_offset, m.g_denc.ptr + sg.out_begin, dL_dinput + sg.in_begin));
-			++g_kernel_launches;
-		}
-	}
+	if (grid_params) plan_param_gradients(m.plan, stream, batch, x, m.g_denc.ptr, mlp.in_width, grads + mlp.n_params, 1.0f);
+	if (dL_dinput) plan_input_gradient(m.plan, stream, batch, x, params + mlp.n_params, m.g_denc.ptr, mlp.in_width, dL_dinput, 1.0f);
 	m.last_stream = stream;
 	m.prof_mark(stream);
 }
@@ -877,9 +724,10 @@ static void training_step(Model& m, cudaStream_t stream, uint32_t batch, uint32_
 	m.prof_mark(stream);
 }
 
-static void finalize_mlp_grads(Model& m, cudaStream_t stream) {
+// fp32 network weight-gradient sums -> fp16 entries of `grads` (what the reference's gradient buffer holds); re-arms the accumulator
+static void finalize_mlp_grads(Model& m, cudaStream_t stream, __half* grads) {
 	if (m.mlp_grads_in_accum) {
-		TCNNB_CUDA_CHECK(launch_mlp_grad_finalize(stream, m.mlp.n_params, m.dw_accum.ptr, m.grads_fp16));
+		TCNNB_CUDA_CHECK(launch_mlp_grad_finalize(stream, m.mlp.n_params, m.dw_accum.ptr, grads));
 		++g_kernel_launches;
 		m.mlp_grads_in_accum = false;
 	}
@@ -905,11 +753,7 @@ static void dp_training_step(Model& m, cudaStream_t stream, uint32_t shard_batch
 		optimizer_step(m, stream);
 		return;
 	}
-	if (m.mlp_grads_in_accum) {  // fp32 network weight-gradient sums -> the fp16 gradient vector (what the reference's buffer holds)
-		TCNNB_CUDA_CHECK(launch_mlp_grad_finalize(stream, m.mlp.n_params, m.dw_accum.ptr, m.grads_fp16));
-		++g_kernel_launches;
-		m.mlp_grads_in_accum = false;
-	}
+	finalize_mlp_grads(m, stream, m.grads_fp16);
 	const size_t chunk = m.n_params_padded / (size_t)d.world, lo = chunk * (size_t)d.rank;
 	if (d.fused) {
 		// Peer-memory engine: [barrier: every rank's gradient vector is complete] -> ONE kernel on this rank's slice that sums the
@@ -1001,12 +845,12 @@ static void module_backward(Model& m, cudaStream_t stream, uint32_t n, float* dL
 		check_batch(n);
 		if (dL_dparams) check_module_ptr(dL_dparams, "dL_dparams");
 		general_backward_pass(m, stream, n, n, x, nullptr, (const __half*)params, (__half*)dL_dparams, (const __half*)dL_doutput, dL_dinput, dL_dparams != nullptr);
-		if (dL_dparams) {
-			TCNNB_CUDA_CHECK(launch_mlp_grad_finalize(stream, m.mlp.n_params, m.dw_accum.ptr, (__half*)dL_dparams));
-			++g_kernel_launches;
-			m.mlp_grads_in_accum = false;
-		}
+		finalize_mlp_grads(m, stream, (__half*)dL_dparams);  // (nothing is accumulated without dL_dparams)
 		return;
+	}
+	// Nothing checks the fused kernel's dL/d(encoded) rows of an Identity encoding; the general path computes this gradient.
+	if (dL_dinput && m.enc_identity) {
+		throw std::runtime_error("module: input gradients through an Identity encoding are not built for configurations the fused kernel runs; the general path (e.g. n_neurons > 64) computes them.");
 	}
 	ModuleIO io;
 	io.params = (const __half*)params;
@@ -1020,7 +864,7 @@ static void module_backward(Model& m, cudaStream_t stream, uint32_t n, float* dL
 	}
 	if (dL_dinput) {
 		// dL/d(input) (cpp_api.cu:104-125 -> NetworkWithInputEncoding::backward -> GridEncoding::backward_impl, grid.h:896-921): the fused
-		// kernel hands out the network's input gradient rows, the stand-alone kernel contracts them with d(encoded)/d(position).
+		// kernel hands out the network's input gradient rows, the plan's grid kernel contracts them with d(encoded)/d(position).
 		m.denc_scratch.resize(std::max(m.denc_scratch.n, (size_t)n * 64));
 		io.dL_dencoded = m.denc_scratch.ptr;
 	}
@@ -1029,26 +873,8 @@ static void module_backward(Model& m, cudaStream_t stream, uint32_t n, float* dL
 		m.mlp_grads_in_accum = false;
 	}
 	training_step(m, stream, n, n, x, nullptr, false, nullptr, &io);
-	// network weight gradients: fp32 sums -> fp16 entries of the caller's array; re-arms the accumulator
-	TCNNB_CUDA_CHECK(launch_mlp_grad_finalize(stream, m.mlp.n_params, m.dw_accum.ptr, io.grads));
-	++g_kernel_launches;
-	m.mlp_grads_in_accum = false;
-	if (dL_dinput) {
-		ensure_levels_dev(m, stream);
-		GridKernelArgs a{};
-		a.n_pos_dims = m.grid.n_pos_dims;
-		a.n_features_per_level = m.grid.n_features_per_level;
-		a.n_levels = m.grid.n_levels;
-		a.interpolation = m.grid.interpolation;
-		a.max_level = 1.0f;
-		a.levels_dev = m.levels_dev.ptr;
-		a.n_elements = n;
-		a.positions = x;
-		a.pos_stride = m.grid.n_pos_dims;
-		a.row_stride = 64;
-		TCNNB_CUDA_CHECK(launch_grid_input_gradient(stream, a, (const __half*)params + m.mlp.n_params, m.denc_scratch.ptr, dL_dinput));
-		++g_kernel_launches;
-	}
+	finalize_mlp_grads(m, stream, io.grads);
+	if (dL_dinput) plan_input_gradient(m.plan, stream, n, x, (const __half*)params + m.mlp.n_params, m.denc_scratch.ptr, 64, dL_dinput, 1.0f);
 }
 
 static void ensure_staging(Model& m, uint32_t batch) {
@@ -1260,7 +1086,7 @@ void* tcnnb_param_gradients(tcnnb_model* m) {
 	// The MLP part is materialised as fp16 on demand (the fused kernel accumulates it in fp32).
 	try {
 		// ordered behind the step that produced the gradients: same stream, and the synchronisation is on that stream only
-		finalize_mlp_grads(m->impl, m->impl.last_stream);
+		finalize_mlp_grads(m->impl, m->impl.last_stream, m->impl.grads_fp16);
 		TCNNB_CUDA_CHECK(cudaStreamSynchronize(m->impl.last_stream));
 	} catch (const std::exception& e) {
 		g_last_error = e.what();
@@ -1271,14 +1097,7 @@ void* tcnnb_param_gradients(tcnnb_model* m) {
 
 int tcnnb_grid_levels(const tcnnb_model* m, uint32_t* n_levels, uint32_t* offsets, float* scales, uint32_t* resolutions) {
 	TCNNB_API_BEGIN
-	const GridConfig& g = m->impl.grid;
-	if (n_levels) *n_levels = g.n_levels;
-	for (uint32_t l = 0; l < g.n_levels; ++l) {
-		if (offsets) offsets[l] = g.offsets[l];
-		if (scales) scales[l] = g.scales[l];
-		if (resolutions) resolutions[l] = (uint32_t)ceilf(g.scales[l]) + 1;
-	}
-	if (offsets) offsets[g.n_levels] = g.offsets[g.n_levels];
+	write_level_table(&m->impl.grid, n_levels, offsets, scales, resolutions);
 	TCNNB_API_END
 }
 
@@ -1698,22 +1517,13 @@ int tcnnb_debug_set(tcnnb_model* m, const char* key, int value) {
 	TCNNB_API_BEGIN
 	const std::string k = key ? key : "";
 	if (k == "binning") m->impl.binning = value != 0;
-	else if (k == "grid_replicas") m->impl.grid_replicas_override = value;
 	else if (k == "general") {
 		// the stand-alone kernels have their own limits (e.g. dL/d(encoded) wider than the layers): only switch when they cover the configuration
 		if (value && !m->impl.general) {
-			MlpBackwardArgs probe{};
-			probe.width = m->impl.mlp.width;
-			probe.in_width = m->impl.mlp.in_width;
-			probe.out_width = m->impl.mlp.padded_out_width;
-			probe.n_hidden_layers = m->impl.mlp.n_hidden_layers;
-			probe.batch_size = 256;
-			probe.dL_dinput = m->impl.grid.n_params == 0 ? nullptr : (__half*)16;
-			const char* why_not = nullptr;
-			if (!mlp_backward_supported(probe, &why_not)) throw std::runtime_error(std::string("tcnnb_debug_set(general): ") + why_not);
+			if (const char* why_not = general_path_unsupported(m->impl)) throw std::runtime_error(std::string("tcnnb_debug_set(general): ") + why_not);
 		}
 		m->impl.force_general = value != 0;
-	}  // general path: copies of the coarse levels' gradient (-1 = automatic)
+	}
 	else throw std::runtime_error("tcnnb_debug_set: unknown key '" + k + "'");
 	TCNNB_API_END
 }

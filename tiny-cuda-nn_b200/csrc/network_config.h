@@ -1,0 +1,72 @@
+// network_config.h -- host-side description of the MLP behind every tier (model.cu: trainer / module tiers; network.cu: the
+// stand-alone network tier): the "network" JSON with the reference's keys, defaults and error texts (src/network.cu:51-141), the
+// parameter layout and the xavier initialisation (fully_fused_mlp.cu:635-672, 868-892).
+#pragma once
+#include "common.cuh"
+#include "host_common.h"
+#include "json_mini.h"
+
+#include <cmath>
+#include <string>
+#include <utility>
+#include <vector>
+
+namespace tcnnb {
+
+struct MlpConfig {
+	std::string otype = "FullyFusedMLP";
+	uint32_t in_width = 0;
+	uint32_t width = 128;
+	uint32_t n_hidden_layers = 5;
+	uint32_t out_width = 0;
+	uint32_t padded_out_width = 0;
+	uint32_t activation = ACT_RELU;
+	uint32_t output_activation = ACT_NONE;
+	uint32_t n_params = 0;
+};
+
+// `in_width`: the (padded) width of the encoding in front of the network; `n_out`: the unpadded output width.
+inline MlpConfig parse_network(const json::Value& net, uint32_t in_width, uint32_t n_out) {
+	MlpConfig c;
+	c.otype = net.value("otype", "MLP");  // src/network.cu:52-54
+	const bool fully_fused = ieq(c.otype, "FullyFusedMLP") || ieq(c.otype, "MegakernelMLP");
+	const bool cutlass = ieq(c.otype, "MLP") || ieq(c.otype, "CutlassMLP");
+	if (!fully_fused && !cutlass) throw std::runtime_error("Invalid network type: " + c.otype);
+	c.width = (uint32_t)net.value("n_neurons", 128.0);
+	c.n_hidden_layers = (uint32_t)net.value("n_hidden_layers", 5.0);
+	c.activation = parse_activation(net.value("activation", "ReLU"));
+	c.output_activation = parse_activation(net.value("output_activation", "None"));
+	// Both otypes run on the same wgmma kernels (there is no separate non-fused network in this library), so both take the fused
+	// kernel's widths; the reference's CutlassMLP accepts any multiple of 8.
+	if (!(c.width == 16 || c.width == 32 || c.width == 64 || c.width == 128)) {
+		throw std::runtime_error("FullyFusedMLP only supports 16, 32, 64, and 128 neurons, but got " + std::to_string(c.width) + ". Use CutlassMLP instead if this is a requirement.");
+	}
+	if (c.n_hidden_layers < 1) throw std::runtime_error("FullyFusedMLP requires at least 1 hidden layer (3 layers in total).");
+	for (uint32_t act : {c.activation, c.output_activation}) {
+		// FullyFusedMLP's activation set (fully_fused_mlp.cu:689-699): Sine and SiLU need stored pre-activations
+		if (act == ACT_SINE || act == ACT_SILU) throw std::runtime_error("Unsupported activation.");
+	}
+	c.in_width = in_width;
+	c.out_width = n_out;
+	c.padded_out_width = next_multiple(n_out, 16u);
+	c.n_params = c.width * c.in_width + (c.n_hidden_layers - 1) * c.width * c.width + c.padded_out_width * c.width;
+	return c;
+}
+
+// Xavier uniform per matrix on the host, sequential draws from `rng` (fully_fused_mlp.cu:868-892, gpu_matrix.h:292-306).
+// `dst`: DEVICE fp32 array of c.n_params elements.
+inline void init_mlp_params(const MlpConfig& c, HostPcg32& rng, float* dst, float scale) {
+	std::vector<float> w(c.n_params);
+	std::vector<std::pair<uint32_t, uint32_t>> mats;  // (rows = fan_out, cols = fan_in)
+	mats.emplace_back(c.width, c.in_width);
+	for (uint32_t i = 0; i + 1 < c.n_hidden_layers; ++i) mats.emplace_back(c.width, c.width);
+	mats.emplace_back(c.padded_out_width, c.width);
+	size_t pos = 0;
+	for (auto& rc : mats) {
+		const float bound = scale * std::sqrt(6.0f / (float)(rc.second + rc.first));
+		for (size_t i = 0; i < (size_t)rc.first * rc.second; ++i) w[pos++] = rng.next_float() * 2.0f * bound - bound;
+	}
+	TCNNB_CUDA_CHECK(cudaMemcpy(dst, w.data(), sizeof(float) * w.size(), cudaMemcpyHostToDevice));
+}
+
+}  // namespace tcnnb
