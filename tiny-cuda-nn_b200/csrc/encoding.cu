@@ -25,7 +25,6 @@ namespace tcnnb {
 struct Encoding {
 	EncodingPlan plan;
 	float max_level = 1.0f;
-	std::string hyperparams_json;
 	uint32_t max_align = 2;             // strictest pointer alignment the kernels need for feature rows / parameters (bytes)
 };
 

@@ -111,7 +111,8 @@ struct DpState {
 
 struct Model {
 	uint32_t n_in = 0, n_out = 0;
-	GridConfig grid;
+	std::string enc_otype;  // the encoding's "otype" as the caller wrote it (hyperparams of encodings other than one grid / Identity)
+	EncodingPlan plan;      // the encoding: segment table, grids, parameter count and padded width
 	MlpConfig mlp;
 	uint32_t loss_type = LOSS_RELATIVE_L2;
 	std::string loss_name = "RelativeL2";
@@ -145,8 +146,7 @@ struct Model {
 	DeviceBuffer<float> dw_accum;   // fp32 MLP weight-gradient accumulator
 	DeviceBuffer<float> scalars;    // [0] = loss sum
 	DeviceBuffer<long long> dbg_clock;  // TCNNB_CLOCKS=<file> in ablation builds: phase stamps of the last ws launch
-	bool enc_identity = false;              // "Identity" encoding instead of a grid (no encoding parameters)
-	float identity_scale = 1.0f, identity_offset = 0.0f;
+	FusedStepParams fused{};                // the fused kernel's per-model arguments (configurations it runs); make_params adds the per-call ones
 	DeviceBuffer<__half> denc_scratch;      // module tier: dL/d(encoded) rows [n][64] handed from the fused kernel to the input-gradient kernel
 	DeviceBuffer<__half> grads_scratch;     // module tier: gradient array when the caller wants dL/d(input) only
 	bool mlp_grads_in_accum = false;
@@ -156,9 +156,6 @@ struct Model {
 	bool general = false;
 	bool force_general = false;  // tcnnb_debug_set("general", 1): run the general path although the fused kernel covers the configuration
 	bool use_general() const { return general || force_general; }
-	bool plan_only = false;      // an encoding other than one grid / Identity (Composite, Frequency, OneBlob, ...): no fused kernel at all
-	EncodingPlan plan;           // segment table of the encoding (general path; module tier: dL/d(input))
-	std::string general_reason;  // which limit of the fused kernel sent this configuration here (hyperparams / diagnostics)
 	DeviceBuffer<__half> g_enc, g_hidden, g_out, g_dy, g_grad_hidden, g_denc, g_dy_act;
 
 	// spatial binning scratch (binning.cu): sorted copies of the batch + permutation
@@ -226,17 +223,11 @@ struct Model {
 		}
 		return e;
 	}
-
-	GridMeta grid_meta() const {
-		GridMeta m{};
-		m.n_levels = grid.n_levels;
-		m.n_features = grid.n_levels * grid.n_features_per_level;
-		m.padded_width = grid.padded_width;
-		m.interpolation = grid.interpolation;
-		for (uint32_t l = 0; l < grid.n_levels; ++l) m.levels[l] = make_level_info(grid, l);
-		return m;
-	}
 };
+
+// Whether the encoding is exactly one encoding of `type` (FEAT_GRID / FEAT_IDENTITY) over all inputs: the two encodings the fused
+// kernel reads. A Composite that nests a single encoding is neither.
+static bool single_encoding(const EncodingPlan& plan, uint32_t type) { return !plan.composite && plan.segs.n == 1 && plan.segs.s[0].type == type; }
 
 // initialize_params(rnd, params_full_precision, scale) of NetworkWithInputEncoding (network_with_input_encoding.h:124-130):
 // network weights first, then the grid table, one pcg32 stream. `dst` is a DEVICE fp32 array of n_params elements.
@@ -254,9 +245,24 @@ static const char* general_path_unsupported(const Model& m) {
 	probe.out_width = m.mlp.padded_out_width;
 	probe.n_hidden_layers = m.mlp.n_hidden_layers;
 	probe.batch_size = 256;
-	probe.dL_dinput = m.grid.n_params == 0 ? nullptr : (__half*)16;  // the encoding's backward pass needs dL/d(encoded)
+	probe.dL_dinput = m.plan.n_params == 0 ? nullptr : (__half*)16;  // the encoding's backward pass needs dL/d(encoded)
 	const char* why_not = nullptr;
 	return mlp_backward_supported(probe, &why_not) ? nullptr : why_not;
+}
+
+// Whether the fused kernel (fused_ws.cu) covers this configuration: nullptr, else the first of its limits that it does not meet.
+static const char* fused_kernel_unsupported(const EncodingPlan& plan, const MlpConfig& mlp, uint32_t n_in) {
+	const GridConfig* grid = single_encoding(plan, FEAT_GRID) ? &plan.grids[0]->cfg : nullptr;
+	if (!grid && !single_encoding(plan, FEAT_IDENTITY)) return "an encoding other than one grid / Identity";
+	if (mlp.width > 64) return "n_neurons > 64";
+	if (mlp.n_hidden_layers > 6) return "n_hidden_layers > 6";
+	if (mlp.padded_out_width != 16) return "more than 16 outputs";
+	if (grid && grid->n_features_per_level != 2) return "n_features_per_level != 2";
+	if (n_in != 2 && n_in != 3) return "input dimensions other than 2 / 3";
+	if (plan.width > 64 || (grid && grid->n_levels > MAX_LEVELS)) return "encoding wider than 64 features";
+	if (fused_ws_smem_bytes(mlp.n_hidden_layers, plan.width, true) > 227 * 1024) return "shared-memory footprint of this depth / encoding width";
+	if (grid && grid->interpolation == INTERP_NEAREST) return "Nearest interpolation";
+	return nullptr;
 }
 
 static void build_model(Model& m, uint32_t n_in, uint32_t n_out, const json::Value& cfg, uint32_t seed, bool module_only = false) {
@@ -334,79 +340,50 @@ static void build_model(Model& m, uint32_t n_in, uint32_t n_out, const json::Val
 	a.optimize_non_matrix_params = opt.value("optimize_non_matrix_params", true);
 	a.skip_zero_grad_non_matrix_params = opt.value("skip_zero_grad_non_matrix_params", true);
 
-	// ---- encoding, padded to the network's alignment (network_with_input_encoding.h:47)
-	const uint32_t alignment = 16;  // FullyFusedMLP / CutlassMLP REQUIRED_ALIGNMENT (src/network.cu:79-98)
+	// ---- encoding, padded to the network's alignment (network_with_input_encoding.h:47; FullyFusedMLP / CutlassMLP REQUIRED_ALIGNMENT,
+	// src/network.cu:79-98). One grid or one Identity (encodings/identity.h:46-67: feature j = x_j * scale + offset, padding features
+	// ONE) can run in the fused kernel; the plan runs every encoding on the general path and the module tier's dL/d(input).
 	const json::Value& enc_cfg = cfg.sub("encoding");
-	if (ieq(enc_cfg.value("otype", "OneBlob"), "Identity")) {
-		// Identity encoding (encodings/identity.h:46-67, src/encoding.cu:77-79): feature j = x_j * scale + offset, the features that pad
-		// the width up to the network's alignment are ONE. No parameters: the memory warps of the fused kernel write the tile rows
-		// directly (BASELINE.json configs[0]: CutlassMLP / FullyFusedMLP 64 x 2 behind Identity).
-		m.enc_identity = true;
-		m.identity_scale = (float)enc_cfg.value("scale", 1.0);
-		m.identity_offset = (float)enc_cfg.value("offset", 0.0);
-		m.grid = GridConfig{};
-		m.grid.otype = "Identity";
-		m.grid.n_pos_dims = n_in;
-		m.grid.n_levels = 0;
-		m.grid.n_params = 0;
-		m.grid.offsets.assign(1, 0u);
-		m.grid.padded_width = next_multiple(n_in, alignment);
-	} else if (plan_detail::is_grid_otype(to_lower(enc_cfg.value("otype", "OneBlob")))) {
-		m.grid = parse_grid(n_in, enc_cfg);
-		m.grid.padded_width = next_multiple(m.grid.n_levels * m.grid.n_features_per_level, alignment);
-	} else {
-		// Composite / Frequency / TriangleWave / OneBlob / SphericalHarmonics (src/encoding.cu:60-120): stand-alone encoding kernels in
-		// front of the stand-alone network kernels. `grid` only carries the totals the rest of the model needs.
-		m.plan_only = true;
-		build_encoding_plan(m.plan, n_in, enc_cfg, alignment);
-		m.grid = GridConfig{};
-		m.grid.otype = enc_cfg.value("otype", "OneBlob");
-		m.grid.n_pos_dims = n_in;
-		m.grid.n_levels = 0;
-		m.grid.n_params = (uint32_t)m.plan.n_params;
-		m.grid.offsets.assign(1, 0u);
-		m.grid.padded_width = m.plan.width;
-	}
+	m.enc_otype = enc_cfg.value("otype", "OneBlob");
+	build_encoding_plan(m.plan, n_in, enc_cfg, 16);
 
 	// ---- network (src/network.cu:51-141)
 	MlpConfig& mlp = m.mlp;
-	mlp = parse_network(cfg.sub("network"), m.grid.padded_width, n_out);
+	mlp = parse_network(cfg.sub("network"), m.plan.width, n_out);
 
-	// ---- which kernels run this configuration. The fused kernel (fused_ws.cu) covers the benchmarked family; everything else the
-	// stand-alone kernels cover takes the general path; the rest fails loudly (no fallback to anything that is not a kernel of this library).
-	if (m.grid.stochastic_interpolation) throw std::runtime_error("tcnn_b200: stochastic_interpolation is not built");
-	{
-		const char* why = nullptr;
-		if (m.plan_only) why = "an encoding other than one grid / Identity";
-		else if (mlp.width > 64) why = "n_neurons > 64";
-		else if (mlp.n_hidden_layers > 6) why = "n_hidden_layers > 6";
-		else if (mlp.padded_out_width != 16) why = "more than 16 outputs";
-		else if (!m.enc_identity && m.grid.n_features_per_level != 2) why = "n_features_per_level != 2";
-		else if (m.grid.n_pos_dims != 2 && m.grid.n_pos_dims != 3) why = "input dimensions other than 2 / 3";
-		else if (m.grid.padded_width > 64 || m.grid.n_levels > MAX_LEVELS) why = "encoding wider than 64 features";
-		else if (fused_ws_smem_bytes(mlp.n_hidden_layers, m.grid.padded_width, true) > 227 * 1024) why = "shared-memory footprint of this depth / encoding width";
-		else if (!m.enc_identity && m.grid.interpolation == INTERP_NEAREST) why = "Nearest interpolation";
-		if (why) {
-			m.general = true;
-			m.general_reason = why;
-			if (const char* why_not = general_path_unsupported(m)) throw std::runtime_error(std::string(why_not) + " (general path of tcnn_b200; the fused kernel does not cover this configuration: " + why + ")");
-			if (!m.enc_identity && !m.plan_only) {
-				const uint32_t F = m.grid.n_features_per_level, D = m.grid.n_pos_dims;
-				if (!(F == 1 || F == 2 || F == 4 || F == 8)) throw std::runtime_error("GridEncoding: n_features_per_level must be 1, 2, 4, or 8.");
-				if (D < 2 || D > 4) throw std::runtime_error("tcnn_b200: grid encodings cover 2, 3 and 4 input dimensions");
-			}
+	// ---- which kernels run this configuration. The fused kernel covers the benchmarked family; everything else the stand-alone
+	// kernels cover takes the general path; the rest fails loudly (no fallback to anything that is not a kernel of this library).
+	if (const char* why = fused_kernel_unsupported(m.plan, mlp, n_in)) {
+		m.general = true;
+		if (const char* why_not = general_path_unsupported(m)) throw std::runtime_error(std::string(why_not) + " (general path of tcnn_b200; the fused kernel does not cover this configuration: " + why + ")");
+	} else {
+		FusedStepParams& p = m.fused;
+		p.ablate = m.ablate;
+		p.grid.padded_width = m.plan.width;
+		if (single_encoding(m.plan, FEAT_GRID)) {
+			const EncodingPlan::Grid& g = *m.plan.grids[0];
+			p.grid.n_levels = g.cfg.n_levels;
+			p.grid.n_features = g.cfg.n_levels * g.cfg.n_features_per_level;
+			p.grid.interpolation = g.cfg.interpolation;
+			std::copy(g.levels.begin(), g.levels.end(), p.grid.levels);
+		} else {
+			p.enc_identity = 1;
+			p.identity_scale = m.plan.segs.s[0].scale;
+			p.identity_offset = m.plan.segs.s[0].offset;
 		}
+		p.width = mlp.width;
+		p.n_hidden_layers = mlp.n_hidden_layers;
+		p.activation = mlp.activation;
+		p.output_activation = mlp.output_activation;
+		p.n_out = n_out;
+		p.n_mlp_params = mlp.n_params;
+		p.loss_type = m.loss_type;
+		p.loss_scale = m.loss_scale;
+		p.dbg_clock = m.dbg_clock.n ? m.dbg_clock.ptr : nullptr;
 	}
 
-	// ---- per-level scales, evaluated on the device like the reference's kernels (common_device.h:886-891)
-	if (!m.enc_identity && !m.plan_only) evaluate_level_scales(m.grid);
-	// one grid / Identity: the segment table of the general path is built for every configuration, so that the general path can run what
-	// the fused kernel also covers (tests: both paths must agree; tcnnb_debug_set("general", 1)) and the module tier's dL/d(input) runs
-	// through it
-	if (!m.plan_only) build_encoding_plan(m.plan, n_in, enc_cfg, alignment);
-
 	// ---- parameter buffers (trainer.h:69-87,489-503)
-	m.n_params = (size_t)mlp.n_params + m.grid.n_params;
+	m.n_params = (size_t)mlp.n_params + m.plan.n_params;
 	// Same order as the reference's single allocation [fp32 master | working fp16 | fp16 gradients]; each region is padded to
 	// a multiple of 512 parameters (never-touched zero entries) so that a data-parallel job can cut it into equal, 16-byte
 	// aligned slices for any world size up to 64 (tcnn_b200/dp.py).
@@ -459,21 +436,8 @@ static void build_model(Model& m, uint32_t n_in, uint32_t n_out, const json::Val
 	}
 }
 
-static FusedStepParams make_params(Model& m, uint32_t batch, uint32_t loss_batch, const float* x, const float* y) {
-	FusedStepParams p{};
-	p.ablate = m.ablate;
-	p.grid = m.grid_meta();
-	p.enc_identity = m.enc_identity ? 1u : 0u;
-	p.identity_scale = m.identity_scale;
-	p.identity_offset = m.identity_offset;
-	p.width = m.mlp.width;
-	p.n_hidden_layers = m.mlp.n_hidden_layers;
-	p.activation = m.mlp.activation;
-	p.output_activation = m.mlp.output_activation;
-	p.n_out = m.n_out;
-	p.n_mlp_params = m.mlp.n_params;
-	p.loss_type = m.loss_type;
-	p.loss_scale = m.loss_scale;
+static FusedStepParams make_params(const Model& m, uint32_t batch, uint32_t loss_batch, const float* x, const float* y) {
+	FusedStepParams p = m.fused;
 	p.batch_size = batch;
 	p.loss_batch_size = loss_batch;
 	p.positions = x;
@@ -489,7 +453,6 @@ static FusedStepParams make_params(Model& m, uint32_t batch, uint32_t loss_batch
 	p.dbg_dy = (__half*)m.taps.dL_doutput;
 	p.dbg_grad_hidden = (__half*)m.taps.grad_hidden;
 	p.dbg_denc = (__half*)m.taps.dL_dencoded;
-	p.dbg_clock = m.dbg_clock.n ? m.dbg_clock.ptr : nullptr;
 	return p;
 }
 
@@ -582,7 +545,7 @@ static void general_forward(Model& m, cudaStream_t stream, uint32_t batch, const
 static void general_backward_pass(Model& m, cudaStream_t stream, uint32_t batch, uint32_t loss_batch, const float* x, const float* y, const __half* params, __half* grads,
                                   const __half* ext_dL_doutput, float* dL_dinput, bool want_param_grads) {
 	const MlpConfig& mlp = m.mlp;
-	const bool grid_params = m.grid.n_params != 0 && want_param_grads;
+	const bool grid_params = m.plan.n_params != 0 && want_param_grads;
 	if (!ext_dL_doutput) TCNNB_CUDA_CHECK(cudaMemsetAsync(m.scalars.ptr, 0, sizeof(float), stream));
 	if (m.mlp_grads_in_accum) {
 		TCNNB_CUDA_CHECK(cudaMemsetAsync(m.dw_accum.ptr, 0, sizeof(float) * mlp.n_params, stream));
@@ -670,8 +633,8 @@ static void training_step(Model& m, cudaStream_t stream, uint32_t batch, uint32_
 	// GradientMode::Overwrite: zero the grid gradient table (grid.h:865-867) and the loss accumulator -- inside the binning pass
 	// when there is one, else as memsets.
 	__half* const grid_grads = grads_base + m.mlp.n_params;
-	const size_t grid_grad_bytes = sizeof(__half) * m.grid.n_params;
-	const bool bin = m.binning && batch >= 16384 && !m.enc_identity;  // spatial order only matters to the table gathers
+	const size_t grid_grad_bytes = sizeof(__half) * m.plan.n_params;
+	const bool bin = m.binning && batch >= 16384 && single_encoding(m.plan, FEAT_GRID);  // spatial order only matters to the table gathers
 	const bool zero_in_binning = bin && (((uintptr_t)grid_grads | grid_grad_bytes) & 15u) == 0;
 	if (!zero_in_binning) {
 		TCNNB_CUDA_CHECK(cudaMemsetAsync(grid_grads, 0, grid_grad_bytes, stream));
@@ -694,17 +657,17 @@ static void training_step(Model& m, cudaStream_t stream, uint32_t batch, uint32_
 	m.prof_mark(stream);
 	// Process the batch in (y, z)-column order: same sums, far fewer distinct memory sectors on the coarse levels (binning.cu).
 	if (bin) {
-		const uint32_t log2_r = binning_log2_resolution(batch, m.grid.n_pos_dims);
+		const uint32_t log2_r = binning_log2_resolution(batch, m.n_in);
 		m.bin_keys.resize(std::max(m.bin_keys.n, 2 * (size_t)batch));
 		m.bin_perm.resize(std::max(m.bin_perm.n, (size_t)batch));
 		{
-			const size_t need = 2 * (size_t)binning_n_bins(log2_r, m.grid.n_pos_dims);
+			const size_t need = 2 * (size_t)binning_n_bins(log2_r, m.n_in);
 			if (m.bin_hist.n != need) {  // layout depends on n_bins: (re)allocate and zero the counters once
 				m.bin_hist.resize(need);
 				m.bin_hist.zero(stream);
 			}
 		}
-		TCNNB_CUDA_CHECK(launch_binning(stream, m.grid.n_pos_dims, batch, x, log2_r, m.bin_keys.ptr, m.bin_hist.ptr, m.bin_perm.ptr, zero_in_binning ? grid_grads : nullptr,
+		TCNNB_CUDA_CHECK(launch_binning(stream, m.n_in, batch, x, log2_r, m.bin_keys.ptr, m.bin_hist.ptr, m.bin_perm.ptr, zero_in_binning ? grid_grads : nullptr,
 		                                zero_in_binning ? grid_grad_bytes : 0, zero_in_binning ? (float*)m.scalars.ptr : nullptr));
 		g_kernel_launches += 3;
 		p.perm = m.bin_perm.ptr;
@@ -713,7 +676,7 @@ static void training_step(Model& m, cudaStream_t stream, uint32_t batch, uint32_
 	if (targets_ready) TCNNB_CUDA_CHECK(cudaStreamWaitEvent(stream, targets_ready, 0));
 	m.wait_pending(stream);  // e.g. the all-gather of the previous data-parallel step: binning above did not need the parameters
 	// one persistent 640-thread CTA per SM (fused_ws.cu)
-	TCNNB_CUDA_CHECK(launch_fused_ws(p, m.grid.n_pos_dims, true, std::min(batch / TILE_M, (uint32_t)m.n_sms), stream));
+	TCNNB_CUDA_CHECK(launch_fused_ws(p, m.n_in, true,std::min(batch / TILE_M, (uint32_t)m.n_sms), stream));
 	++g_kernel_launches;
 	m.last_stream = stream;
 	m.prof_mark(stream);
@@ -748,7 +711,7 @@ static void dp_training_step(Model& m, cudaStream_t stream, uint32_t shard_batch
 		return;
 	}
 	if (!d.shard_optimizer) {
-		TCNNB_NCCL_CHECK(n.AllReduce(m.grads_fp16 + m.mlp.n_params, m.grads_fp16 + m.mlp.n_params, m.grid.n_params, ncclHalf, ncclSum, d.comm_grads, stream));
+		TCNNB_NCCL_CHECK(n.AllReduce(m.grads_fp16 + m.mlp.n_params, m.grads_fp16 + m.mlp.n_params, m.plan.n_params, ncclHalf, ncclSum, d.comm_grads, stream));
 		TCNNB_NCCL_CHECK(n.AllReduce(m.dw_accum.ptr, m.dw_accum.ptr, m.mlp.n_params, ncclFloat, ncclSum, d.comm_grads, stream));
 		optimizer_step(m, stream);
 		return;
@@ -790,7 +753,7 @@ static void dp_reduce_loss(Model& m, cudaStream_t stream) {
 
 static void launch_inference(Model& m, const FusedStepParams& p, uint32_t batch, cudaStream_t stream) {
 	// the warp-specialised kernel without its backward half (measured 0.0885 ms vs 0.127 ms for the bulk-synchronous kernel it replaced)
-	TCNNB_CUDA_CHECK(launch_fused_ws(p, m.grid.n_pos_dims, false, std::min(batch / TILE_M, (uint32_t)m.n_sms), stream));
+	TCNNB_CUDA_CHECK(launch_fused_ws(p, m.n_in, false,std::min(batch / TILE_M, (uint32_t)m.n_sms), stream));
 	++g_kernel_launches;
 	m.last_stream = stream;
 }
@@ -849,7 +812,7 @@ static void module_backward(Model& m, cudaStream_t stream, uint32_t n, float* dL
 		return;
 	}
 	// Nothing checks the fused kernel's dL/d(encoded) rows of an Identity encoding; the general path computes this gradient.
-	if (dL_dinput && m.enc_identity) {
+	if (dL_dinput && single_encoding(m.plan, FEAT_IDENTITY)) {
 		throw std::runtime_error("module: input gradients through an Identity encoding are not built for configurations the fused kernel runs; the general path (e.g. n_neurons > 64) computes them.");
 	}
 	ModuleIO io;
@@ -964,24 +927,25 @@ static float host_step_wait(Model& m, uint64_t ticket) {
 static std::string make_hyperparams(const Model& m) {
 	json::Value root = json::Value::object();
 	json::Value& enc = root["encoding"];
-	if (m.enc_identity) {
+	if (single_encoding(m.plan, FEAT_GRID)) {
+		const GridConfig& g = m.plan.grids[0]->cfg;
+		enc["otype"] = json::Value::string("Grid");
+		enc["type"] = json::Value::string(g.grid_type == GRID_HASH ? "Hash" : (g.grid_type == GRID_DENSE ? "Dense" : "Tiled"));
+		enc["n_levels"] = json::Value::number(g.n_levels);
+		enc["n_features_per_level"] = json::Value::number(g.n_features_per_level);
+		enc["base_resolution"] = json::Value::number(g.base_resolution);
+		enc["log2_hashmap_size"] = json::Value::number(g.log2_hashmap_size);
+		enc["per_level_scale"] = json::Value::number(g.per_level_scale);
+		enc["interpolation"] = json::Value::string(g.interpolation == INTERP_LINEAR ? "Linear" : (g.interpolation == INTERP_SMOOTHSTEP ? "Smoothstep" : "Nearest"));
+		enc["hash"] = json::Value::string("CoherentPrime");
+	} else if (single_encoding(m.plan, FEAT_IDENTITY)) {
 		enc["otype"] = json::Value::string("Identity");
-		enc["scale"] = json::Value::number(m.identity_scale);
-		enc["offset"] = json::Value::number(m.identity_offset);
-	} else if (m.plan_only) {
-		enc["otype"] = json::Value::string(m.grid.otype);
+		enc["scale"] = json::Value::number(m.plan.segs.s[0].scale);
+		enc["offset"] = json::Value::number(m.plan.segs.s[0].offset);
+	} else {
+		enc["otype"] = json::Value::string(m.enc_otype);
 		enc["n_nested"] = json::Value::number(m.plan.segs.n);
 		enc["n_output_dims"] = json::Value::number(m.plan.width);
-	} else {
-	enc["otype"] = json::Value::string("Grid");
-	enc["type"] = json::Value::string(m.grid.grid_type == GRID_HASH ? "Hash" : (m.grid.grid_type == GRID_DENSE ? "Dense" : "Tiled"));
-	enc["n_levels"] = json::Value::number(m.grid.n_levels);
-	enc["n_features_per_level"] = json::Value::number(m.grid.n_features_per_level);
-	enc["base_resolution"] = json::Value::number(m.grid.base_resolution);
-	enc["log2_hashmap_size"] = json::Value::number(m.grid.log2_hashmap_size);
-	enc["per_level_scale"] = json::Value::number(m.grid.per_level_scale);
-	enc["interpolation"] = json::Value::string(m.grid.interpolation == INTERP_LINEAR ? "Linear" : (m.grid.interpolation == INTERP_SMOOTHSTEP ? "Smoothstep" : "Nearest"));
-	enc["hash"] = json::Value::string("CoherentPrime");
 	}
 	json::Value& net = root["network"];
 	net["otype"] = json::Value::string("FullyFusedMLP");
@@ -1001,7 +965,7 @@ static std::string make_hyperparams(const Model& m) {
 	opt["l2_reg"] = json::Value::number(m.adam.l2_reg);
 	root["n_params"] = json::Value::number((double)m.n_params);
 	root["n_mlp_params"] = json::Value::number(m.mlp.n_params);
-	root["encoded_width"] = json::Value::number(m.grid.padded_width);
+	root["encoded_width"] = json::Value::number(m.plan.width);
 	return json::dump(root);
 }
 
@@ -1076,7 +1040,7 @@ uint64_t tcnnb_n_mlp_params(const tcnnb_model* m) { return m->impl.mlp.n_params;
 uint32_t tcnnb_n_input_dims(const tcnnb_model* m) { return m->impl.n_in; }
 uint32_t tcnnb_n_output_dims(const tcnnb_model* m) { return m->impl.n_out; }
 uint32_t tcnnb_padded_output_width(const tcnnb_model* m) { return m->impl.mlp.padded_out_width; }
-uint32_t tcnnb_encoded_width(const tcnnb_model* m) { return m->impl.grid.padded_width; }
+uint32_t tcnnb_encoded_width(const tcnnb_model* m) { return m->impl.plan.width; }
 float* tcnnb_params_full_precision(tcnnb_model* m) { return m->impl.params_fp32; }
 void* tcnnb_params(tcnnb_model* m) { return m->impl.params_fp16; }
 float* tcnnb_mlp_gradient_accumulator(tcnnb_model* m) { return m->impl.dw_accum.ptr; }
@@ -1095,9 +1059,11 @@ void* tcnnb_param_gradients(tcnnb_model* m) {
 	return m->impl.grads_fp16;
 }
 
+// Level table of the grid when the encoding is one grid; n_levels = 0 for any other encoding, a Composite of one grid included.
 int tcnnb_grid_levels(const tcnnb_model* m, uint32_t* n_levels, uint32_t* offsets, float* scales, uint32_t* resolutions) {
 	TCNNB_API_BEGIN
-	write_level_table(&m->impl.grid, n_levels, offsets, scales, resolutions);
+	const EncodingPlan& plan = m->impl.plan;
+	write_level_table(single_encoding(plan, FEAT_GRID) ? &plan.grids[0]->cfg : nullptr, n_levels, offsets, scales, resolutions);
 	TCNNB_API_END
 }
 

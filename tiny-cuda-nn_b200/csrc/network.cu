@@ -24,7 +24,6 @@ struct Network {
 	MlpConfig cfg;
 	int n_sms = 132;
 	long long* dbg_clock = nullptr;  // profiling only (tcnnb_network_debug_clocks)
-	std::string hyperparams_json;
 	// scratch of the backward pass (grown on demand, reused): g_l rows, dL/d(output) through the output activation, fp32 weight-gradient
 	// sums, and -- module tier, fp32 inputs -- the Identity-encoded input rows, the recomputed activations and dL/d(encoded input)
 	DeviceBuffer<__half> grad_hidden, grad_output, enc_input, hidden, output, grad_input;
