@@ -141,6 +141,13 @@ int tcnnb_encoding_forward(tcnnb_encoding* e, tcnnb_stream stream, uint32_t n_el
  * either result pointer may be null. params_dev is needed for dL_dinput only. */
 int tcnnb_encoding_backward(tcnnb_encoding* e, tcnnb_stream stream, uint32_t n_elements, float* dL_dinput_dev, const void* dL_doutput_dev, void* dL_dparams_dev, const float* input_dev,
                             const void* params_dev);
+/* backward_backward_input (cpp_api.h:80; GridEncoding, grid.h:910-1042): the derivatives of a loss on dL_dinput, given
+ * dL_ddLdinput fp32 [n][n_input_dims] and the dL_doutput fp16 [n][n_output_dims] of the first backward pass. Every non-null result is
+ * OVERWRITTEN: dL_dparams fp16 [n_params], dL_ddLdoutput fp16 [n][n_output_dims], dL_dinput fp32 [n][n_input_dims]. dL_doutput is
+ * needed for dL_dparams and dL_dinput, params_dev for dL_ddLdoutput and dL_dinput. Grid / HashGrid / DenseGrid / TiledGrid on their
+ * own only: every other encoding (Composite included) fails with "<name> does not support double backward." */
+int tcnnb_encoding_backward_backward_input(tcnnb_encoding* e, tcnnb_stream stream, uint32_t n_elements, const float* dL_ddLdinput_dev, const float* input_dev,
+                                           const void* dL_doutput_dev, void* dL_dparams_dev, void* dL_ddLdoutput_dev, float* dL_dinput_dev, const void* params_dev);
 
 /* ---- network tier: a FullyFusedMLP on its own -------------------------------------------------------------------------------
  * tcnn::create_network<T>(json) (network.h; src/network.cu:51-141; the object benchmarks/mlp/bench_mlp_ours.cu drives) and

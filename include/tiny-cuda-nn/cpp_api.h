@@ -7,8 +7,10 @@
  * [n][n_output_dims()] with n_output_dims() the PADDED width; params / dL_dparams caller-owned arrays of n_params() elements in
  * param_precision() (fp16); gradients are OVERWRITTEN; a null result pointer means "do not compute"; factories return owning raw
  * pointers. Differences, by design: forward() keeps no activations (backward recomputes the forward pass inside the fused kernel),
- * so the returned Context only marks "a forward pass was made"; jit fusion does not exist (the fused kernel is the product);
- * backward_backward_input throws. */
+ * so the returned Context only marks "a forward pass was made"; jit fusion does not exist (the fused kernel is the product).
+ * backward_backward_input is built where the reference builds it, for the grid encodings of create_encoding (recomputed from the
+ * input and the parameters, no forward context needed); every other encoding reports "<name> does not support double backward."
+ * and the network modules throw. */
 #pragma once
 #if __has_include(<json/json.hpp>)
 #include <json/json.hpp>
@@ -192,8 +194,9 @@ public:
 	void backward(cudaStream_t stream, const Context&, uint32_t n, float* dL_dinput, const void* dL_doutput, void* dL_dparams, const float* input, const void*, const void* params) override {
 		TCNNB_CPP_CHECK(tcnnb_encoding_backward(m_h, (tcnnb_stream)stream, n, dL_dinput, dL_doutput, dL_dparams, input, params));
 	}
-	void backward_backward_input(cudaStream_t, const Context&, uint32_t, const float*, const float*, const void*, void*, void*, float*, const void*) override {
-		throw std::runtime_error{"tcnn_b200: second-order derivatives (backward_backward_input) are outside the built path"};
+	void backward_backward_input(cudaStream_t stream, const Context&, uint32_t n, const float* dL_ddLdinput, const float* input, const void* dL_doutput, void* dL_dparams, void* dL_ddLdoutput,
+	                             float* dL_dinput, const void* params) override {
+		TCNNB_CPP_CHECK(tcnnb_encoding_backward_backward_input(m_h, (tcnnb_stream)stream, n, dL_ddLdinput, input, dL_doutput, dL_dparams, dL_ddLdoutput, dL_dinput, params));
 	}
 	uint32_t n_input_dims() const override { return tcnnb_encoding_n_input_dims(m_h); }
 	uint32_t n_output_dims() const override { return tcnnb_encoding_n_output_dims(m_h); }

@@ -6,6 +6,8 @@
 // "SphericalHarmonics" and "Composite" of those (src/encoding.cu:60-120):
 //   forward / inference   fp32 inputs [n][n_input_dims] -> fp16 features [n][n_output_dims]
 //   backward              dL_dparams (fp16, OVERWRITTEN; grids only) and / or dL_dinput fp32 from dL_doutput
+//   backward_backward_input  second-order derivatives of a single grid (grid.h:910-1042, grid_bwd_bwd.cu); every other
+//                         encoding throws "<name> does not support double backward." as the reference (object.h:468-482)
 //   initialize_params     grids: U(-1e-4, 1e-4) * scale from pcg32{seed}, nested encodings one after the other (grid.h:1076-1079)
 // The configuration is resolved into a segment table (encoding_plan.h); grids run grid_kernels.cu, everything else
 // feature_encodings.cu. Parameters are CALLER-owned. Only the fp16 build of the reference is mirrored (Precision::Fp32 is rejected).
@@ -117,6 +119,24 @@ int tcnnb_encoding_backward(tcnnb_encoding* e, tcnnb_stream stream, uint32_t n_e
 	const __half* dy = (const __half*)dL_doutput_dev;
 	if (dL_dparams_dev) plan_param_gradients(plan, s, n_elements, input_dev, dy, plan.width, (__half*)dL_dparams_dev, enc.max_level);  // GradientMode::Overwrite (src/cpp_api.cu:115)
 	if (dL_dinput_dev) plan_input_gradient(plan, s, n_elements, input_dev, (const __half*)params_dev, dy, plan.width, dL_dinput_dev, enc.max_level);
+	TCNNB_API_END
+}
+
+int tcnnb_encoding_backward_backward_input(tcnnb_encoding* e, tcnnb_stream stream, uint32_t n_elements, const float* dL_ddLdinput_dev, const float* input_dev,
+                                           const void* dL_doutput_dev, void* dL_dparams_dev, void* dL_ddLdoutput_dev, float* dL_dinput_dev, const void* params_dev) {
+	TCNNB_API_BEGIN
+	Encoding& enc = e->impl;
+	EncodingPlan& plan = enc.plan;
+	check_batch(n_elements);
+	check_ptr(input_dev, "input", 4);
+	check_ptr(dL_ddLdinput_dev, "dL_ddLdinput", 4);
+	if (dL_dparams_dev || dL_dinput_dev) check_ptr(dL_doutput_dev, "dL_doutput", enc.max_align);
+	if (dL_dparams_dev && plan.n_params) check_ptr(dL_dparams_dev, "dL_dparams", enc.max_align);
+	if (dL_ddLdoutput_dev) check_ptr(dL_ddLdoutput_dev, "dL_ddLdoutput", enc.max_align);
+	if (dL_dinput_dev) check_ptr(dL_dinput_dev, "dL_dinput", 4);
+	if ((dL_ddLdoutput_dev || dL_dinput_dev) && plan.n_params) check_ptr(params_dev, "params", enc.max_align);
+	plan_backward_backward_input(plan, (cudaStream_t)stream, n_elements, input_dev, (const __half*)params_dev, (const __half*)dL_doutput_dev, plan.width, dL_ddLdinput_dev,
+	                             (__half*)dL_dparams_dev, (__half*)dL_ddLdoutput_dev, dL_dinput_dev, enc.max_level);
 	TCNNB_API_END
 }
 

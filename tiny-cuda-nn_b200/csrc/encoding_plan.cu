@@ -68,6 +68,38 @@ void plan_input_gradient(const EncodingPlan& plan, cudaStream_t stream, uint32_t
 	}
 }
 
+void plan_backward_backward_input(EncodingPlan& plan, cudaStream_t stream, uint32_t n, const float* x, const __half* params, const __half* dL_doutput,
+                                  uint32_t row_stride, const float* dL_ddLdinput, __half* dL_dparams, __half* dL_ddLdoutput, float* dL_dinput, float max_level) {
+	if (plan.composite || plan.segs.n != 1 || plan.grids.size() != 1) {
+		// the reference implements double backward for grid encodings only (object.h:468-482)
+		static const char* const names[] = {"Identity", "Frequency", "TriangleWave", "OneBlob", "SphericalHarmonics", "Grid"};
+		const uint32_t type = plan.segs.n ? plan.segs.s[0].type : 0u;
+		const std::string name = plan.composite ? "Composite" : (type < sizeof(names) / sizeof(names[0]) ? names[type] : "Encoding");
+		throw std::runtime_error(name + " does not support double backward.");
+	}
+	const EncodingPlan::Grid& g = *plan.grids.front();
+	const FeatureSegment& sg = plan.segs.s[g.segment];
+	GridKernelArgs a = plan_grid_args(g, n, x + sg.in_begin, plan.n_in, row_stride, max_level);
+	a.pad_cols = sg.n_pad;
+	float* tmp = nullptr;
+	if (dL_dparams) {
+		TCNNB_CUDA_CHECK(cudaMemsetAsync(dL_dparams, 0, sizeof(__half) * plan.n_params, stream));  // GradientMode::Overwrite (grid.h:959-961)
+		if (g.cfg.n_features_per_level == 1) {
+			grow(plan.grad_fp32, g.cfg.n_params);
+			tmp = plan.grad_fp32.ptr;
+			TCNNB_CUDA_CHECK(cudaMemsetAsync(tmp, 0, sizeof(float) * g.cfg.n_params, stream));
+		}
+	}
+	if (!dL_dparams && !dL_ddLdoutput && !dL_dinput) return;
+	const __half* table = params ? params + g.param_offset : nullptr;
+	TCNNB_CUDA_CHECK(launch_grid_backward_backward_input(stream, a, table, dL_doutput ? dL_doutput + sg.out_begin : nullptr, dL_ddLdinput + sg.in_begin,
+	                                                     dL_dparams ? dL_dparams + g.param_offset : nullptr, tmp, g.cfg.n_params,
+	                                                     dL_ddLdoutput ? dL_ddLdoutput + sg.out_begin : nullptr, dL_dinput ? dL_dinput + sg.in_begin : nullptr));
+	// the kernel, and the fp32 -> fp16 cast of the F == 1 parameter gradient; Nearest scatters nothing
+	const bool scatter = dL_dparams && g.cfg.interpolation != INTERP_NEAREST;
+	g_kernel_launches += ((scatter || dL_ddLdoutput || dL_dinput) ? 1 : 0) + (scatter && g.cfg.n_features_per_level == 1 ? 1 : 0);
+}
+
 void init_plan_params(const EncodingPlan& plan, HostPcg32& rng, float* dst, float scale) {
 	for (auto& g : plan.grids) {
 		TCNNB_CUDA_CHECK(launch_random_uniform(nullptr, rng.device(), g->cfg.n_params, dst + g->param_offset, -1e-4f * scale, 1e-4f * scale));

@@ -202,6 +202,11 @@ void plan_param_gradients(EncodingPlan& plan, cudaStream_t stream, uint32_t n, c
 // dL_dx [n][plan.n_in] fp32 (OVERWRITTEN) = dL/d(encoded) contracted with d(encoded)/d(position)
 void plan_input_gradient(const EncodingPlan& plan, cudaStream_t stream, uint32_t n, const float* x, const __half* params, const __half* dL_dencoded, uint32_t row_stride,
                          float* dL_dx, float max_level);
+// Second-order derivatives of a plan that is ONE grid (GridEncoding::backward_backward_input; anything else throws "... does not
+// support double backward", object.h:468-482) from dL_ddLdinput [n][plan.n_in] fp32 and dL_doutput [n][row_stride] fp16. Each
+// non-null result is OVERWRITTEN: dL_dparams fp16 [n_params], dL_ddLdoutput fp16 [n][row_stride], dL_dinput fp32 [n][plan.n_in].
+void plan_backward_backward_input(EncodingPlan& plan, cudaStream_t stream, uint32_t n, const float* x, const __half* params, const __half* dL_doutput,
+                                  uint32_t row_stride, const float* dL_ddLdinput, __half* dL_dparams, __half* dL_ddLdoutput, float* dL_dinput, float max_level);
 // Grid tables U(-1e-4, 1e-4) * scale from `rng`, nested grids one after the other (grid.h:1076-1079, composite.h initialize_params).
 // `dst`: DEVICE fp32 array of plan.n_params elements.
 void init_plan_params(const EncodingPlan& plan, HostPcg32& rng, float* dst, float scale);

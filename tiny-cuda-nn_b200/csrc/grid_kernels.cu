@@ -20,62 +20,7 @@ namespace tcnnb {
 
 namespace {
 
-template <uint32_t F>
-struct Entry {
-	__half v[F];
-};
-
-template <uint32_t F>
-__device__ __forceinline__ Entry<F> load_entry(const __half* __restrict__ p) {
-	Entry<F> e;
-	if (F == 1) {
-		e.v[0] = __ldg(p);
-	} else if (F == 2) {
-		*reinterpret_cast<uint32_t*>(e.v) = __ldg(reinterpret_cast<const uint32_t*>(p));
-	} else if (F == 4) {
-		*reinterpret_cast<uint2*>(e.v) = __ldg(reinterpret_cast<const uint2*>(p));
-	} else {
-		*reinterpret_cast<uint4*>(e.v) = __ldg(reinterpret_cast<const uint4*>(p));
-	}
-	return e;
-}
-
-template <uint32_t F>
-__device__ __forceinline__ void store_entry(__half* p, const Entry<F>& e) {
-	if (F == 1) {
-		p[0] = e.v[0];
-	} else if (F == 2) {
-		*reinterpret_cast<uint32_t*>(p) = *reinterpret_cast<const uint32_t*>(e.v);
-	} else if (F == 4) {
-		*reinterpret_cast<uint2*>(p) = *reinterpret_cast<const uint2*>(e.v);
-	} else {
-		*reinterpret_cast<uint4*>(p) = *reinterpret_cast<const uint4*>(e.v);
-	}
-}
-
-// one reduction per corner: f16x2, v2.f16x2 or v4.f16x2 (an entry of F fp16 is F * 2 bytes and aligned to that)
-template <uint32_t F>
-__device__ __forceinline__ void red_entry(__half* p, const Entry<F>& e) {
-	const uint32_t* w = reinterpret_cast<const uint32_t*>(e.v);
-	if (F == 2) {
-		asm volatile("red.relaxed.gpu.global.add.noftz.f16x2 [%0], %1;" ::"l"(p), "r"(w[0]) : "memory");
-	} else if (F == 4) {
-		asm volatile("red.relaxed.gpu.global.add.noftz.v2.f16x2 [%0], {%1, %2};" ::"l"(p), "r"(w[0]), "r"(w[1]) : "memory");
-	} else if (F == 8) {
-		asm volatile("red.relaxed.gpu.global.add.noftz.v4.f16x2 [%0], {%1, %2, %3, %4};" ::"l"(p), "r"(w[0]), "r"(w[1]), "r"(w[2]), "r"(w[3]) : "memory");
-	}
-}
-
-template <uint32_t D>
-__device__ __forceinline__ void load_position(const float* __restrict__ positions, uint32_t stride, uint32_t i, float (&x)[D]) {
-#pragma unroll
-	for (uint32_t d = 0; d < D; ++d) x[d] = __ldg(positions + (size_t)i * stride + d);
-}
-
-__device__ __forceinline__ float active_levels(const GridKernelArgs& a) {
-	// max_level = (max_level * num_grid_features) / N_FEATURES_PER_LEVEL (grid.h:69-73)
-	return (a.max_level * (float)(a.n_levels * a.n_features_per_level)) / (float)a.n_features_per_level;
-}
+__device__ __forceinline__ float active_levels(const GridKernelArgs& a) { return grid_active_levels(a.max_level, a.n_levels, a.n_features_per_level); }
 
 template <uint32_t D, uint32_t F>
 __global__ void grid_forward_kernel(const GridKernelArgs a, const __half* __restrict__ table, __half* __restrict__ encoded) {

@@ -41,5 +41,13 @@ cudaError_t launch_grid_forward(cudaStream_t stream, const GridKernelArgs& a, co
 cudaError_t launch_grid_backward(cudaStream_t stream, const GridKernelArgs& a, const __half* dL_dy, __half* grad_table, float* tmp_fp32, uint32_t n_params);
 // dL_dx [n][pos_stride] fp32 (first D columns) = sum over features of dL_dy * d(encoded)/d(position)                                           grid.h:170-212,322-350
 cudaError_t launch_grid_input_gradient(cudaStream_t stream, const GridKernelArgs& a, const __half* table, const __half* dL_dy, float* dL_dx);
+// Second-order derivatives (grid_bwd_bwd.cu; grid.h:351-655,910-1042) from dL_ddLdx [n][pos_stride] fp32 (first D columns) and
+// dL_dy [n][row_stride] fp16; each of the three results is computed when its pointer is non-null:
+//   grad_table (fp16, n_params, accumulated INTO: the caller zeroes it; F == 1 accumulates in `tmp_fp32`, zeroed by the caller, and casts)
+//   dL_ddLdy [n][row_stride] fp16 (OVERWRITTEN, pad_cols behind the features zeroed)
+//   dL_dx [n][pos_stride] fp32 (first D columns, OVERWRITTEN)
+// One launch (plus the cast when F == 1). Replicated scatter (replica_scratch) is not used.
+cudaError_t launch_grid_backward_backward_input(cudaStream_t stream, const GridKernelArgs& a, const __half* table, const __half* dL_dy, const float* dL_ddLdx,
+                                                __half* grad_table, float* tmp_fp32, uint32_t n_params, __half* dL_ddLdy, float* dL_dx);
 
 }  // namespace tcnnb

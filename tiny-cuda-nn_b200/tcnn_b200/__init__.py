@@ -79,6 +79,7 @@ ABI = [
     ("tcnnb_encoding_initialize_params", _int, [_vp, _u64, _vp, ctypes.c_float]),
     ("tcnnb_encoding_forward", _int, [_vp, _vp, _u32, _vp, _vp, _vp]),
     ("tcnnb_encoding_backward", _int, [_vp, _vp, _u32, _vp, _vp, _vp, _vp, _vp]),
+    ("tcnnb_encoding_backward_backward_input", _int, [_vp, _vp, _u32, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     ("tcnnb_network_create", _int, [_u32, _u32, ctypes.c_char_p, ctypes.POINTER(_vp)]),
     ("tcnnb_network_destroy", None, [_vp]),
     ("tcnnb_network_n_params", _u64, [_vp]),
@@ -461,6 +462,10 @@ class Module:
                                             grads.data_ptr() if want_param_grad else None, inputs.data_ptr(), output.data_ptr() if output is not None else None, params.data_ptr()))
         return (grads, dinput) if want_input_grad else grads
 
+    def bwd_bwd_input(self, *args, **kwargs):
+        """Second-order derivatives are built for the grid encodings alone (Encoding.bwd_bwd_input), as in the reference."""
+        raise TcnnError("NetworkWithInputEncoding does not support double backward.")
+
     def close(self):
         if self._h:
             load().tcnnb_destroy(self._h)
@@ -521,6 +526,21 @@ class Encoding:
         _check(load().tcnnb_encoding_backward(self._h, _stream_handle(stream), x.shape[0], gx.data_ptr() if want_input else None, dL_doutput.data_ptr(),
                                               gp.data_ptr() if want_params else None, x.data_ptr(), params16.data_ptr()))
         return gp, gx
+
+    def bwd_bwd_input(self, x, params16, dL_ddLdinput, dL_doutput, want_doutput=True, want_params=True, want_input=False, stream=None):
+        """Module::backward_backward_input (cpp_api.h:80) of a grid encoding: the derivatives of a loss on dL_dinput, given
+        dL_ddLdinput fp32 [n][n_input_dims] and the first backward pass's dL_doutput fp16 [n][n_output_dims]
+        -> (dL_ddLdoutput fp16 [n][n_output_dims] or None, dL_dparams fp16 [n_params] or None, dL_dinput fp32 [n][n_input_dims] or None).
+        Other encodings raise "<name> does not support double backward." """
+        import torch
+
+        dd = torch.empty(x.shape[0], self.n_output_dims, dtype=torch.float16, device=x.device) if want_doutput else None
+        gp = torch.empty(self.n_params, dtype=torch.float16, device=x.device) if want_params else None
+        gx = torch.empty(x.shape[0], self.n_input_dims, dtype=torch.float32, device=x.device) if want_input else None
+        _check(load().tcnnb_encoding_backward_backward_input(self._h, _stream_handle(stream), x.shape[0], dL_ddLdinput.data_ptr(), x.data_ptr(),
+                                                             dL_doutput.data_ptr() if dL_doutput is not None else None, gp.data_ptr() if want_params else None,
+                                                             dd.data_ptr() if want_doutput else None, gx.data_ptr() if want_input else None, params16.data_ptr()))
+        return dd, gp, gx
 
     def close(self):
         if self._h:
@@ -605,6 +625,10 @@ class Network:
         _check(load().tcnnb_network_module_backward(self._h, _stream_handle(stream), n, dx.data_ptr() if dx is not None else None, dL_doutput16.data_ptr(),
                                                     dp.data_ptr() if dp is not None else None, x32.data_ptr(), params16.data_ptr()))
         return dx, dp
+
+    def bwd_bwd_input(self, *args, **kwargs):
+        """Second-order derivatives are built for the grid encodings alone (Encoding.bwd_bwd_input), as in the reference."""
+        raise TcnnError("Network does not support double backward.")
 
     def inference(self, x32, params16, stream=None):
         """fp32 [n][n_input_dims] through the Identity encoding -> fp32 [n][n_output_dims]."""

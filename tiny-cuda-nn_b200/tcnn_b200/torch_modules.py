@@ -12,7 +12,9 @@ Same conventions as the reference binding: parameters are an fp32 `torch.nn.Para
 256 (modules.py:222-226); gradients w.r.t. the output are multiplied by the loss scale (128 for fp16) before the native
 backward pass and the parameter / input gradients divided by it afterwards (modules.py:166-171); the padded output columns are
 sliced away (modules.py:233). Gradients w.r.t. the input positions are delivered when the input requires grad (modules.py:153-160).
-Not supported: second-order terms (bwd_bwd_input).
+Second-order terms (modules.py:161-200): the backward pass of `Encoding` is itself differentiable under `create_graph=True` for the
+grid encodings (an eikonal loss on dL/dx reaches the grid table, the input and dL/d(output)); other encodings raise
+"... does not support double backward". The network modules deliver first-order gradients only.
 
 This file is glue: the work happens in libtcnn_b200 (fused sm_90a kernels) behind `tcnnb_module_*`, `tcnnb_encoding_*`, `tcnnb_network_*`.
 """
@@ -44,6 +46,10 @@ class _ModuleFunction(torch.autograd.Function):
         want_input, want_params = ctx.needs_input_grad[1], ctx.needs_input_grad[2]
         if not (want_input or want_params):
             return None, None, None, None
+        if isinstance(ctx.native, _NativeEncoding) and torch.is_grad_enabled():
+            # backward with create_graph=True: the gradients become differentiable (a loss on dL_dinput, e.g. an eikonal term)
+            dinput, grads = _EncodingBackwardFunction.apply(ctx.native, ctx.loss_scale, doutput, inputs, params, want_input, want_params)
+            return None, dinput, grads, None
         with torch.no_grad():
             scaled = (doutput.to(torch.float32) * ctx.loss_scale).to(torch.float16).contiguous()
             if isinstance(ctx.native, _NativeEncoding):
@@ -55,6 +61,39 @@ class _ModuleFunction(torch.autograd.Function):
             grads = (grads.to(torch.float32) / ctx.loss_scale).to(params.dtype) if grads is not None else None
             dinput = (dinput / ctx.loss_scale).to(inputs.dtype) if dinput is not None else None
         return None, dinput, grads, None
+
+
+class _EncodingBackwardFunction(torch.autograd.Function):
+    """The encoding's backward pass as a differentiable function of (doutput, inputs, params) -- modules.py:161-200. Its own backward
+    is Module::backward_backward_input: grid encodings only, every other encoding raises "... does not support double backward"."""
+
+    @staticmethod
+    def forward(ctx, native, loss_scale, doutput, inputs, params, want_input, want_params):
+        ctx.set_materialize_grads(False)
+        scaled = (doutput.to(torch.float32) * loss_scale).to(torch.float16).contiguous()
+        grads, dinput = native.bwd(inputs, params, scaled, want_params=want_params, want_input=want_input)
+        grads = (grads.to(torch.float32) / loss_scale).to(params.dtype) if grads is not None else None
+        dinput = (dinput / loss_scale).to(inputs.dtype) if dinput is not None else None
+        ctx.save_for_backward(inputs, params, scaled)
+        ctx.native = native
+        ctx.loss_scale = loss_scale
+        return dinput, grads
+
+    @staticmethod
+    def backward(ctx, d_dinput, d_dparams):
+        # d_dparams (a loss on the parameter gradient) is not propagated, as in the reference ("x d(dL_dparam)_d(...)")
+        want_doutput, want_input, want_params = ctx.needs_input_grad[2], ctx.needs_input_grad[3], ctx.needs_input_grad[4]
+        if d_dinput is None or not (want_doutput or want_input or want_params):
+            return None, None, None, None, None, None, None
+        inputs, params, scaled = ctx.saved_tensors
+        with torch.no_grad():
+            # dL_doutput reached the native call multiplied by the loss scale: the parameter and input results carry it, the
+            # dL_doutput result (a function of d_dinput alone) does not
+            ddoutput, grads, dinput = ctx.native.bwd_bwd_input(inputs, params, d_dinput.to(torch.float32).contiguous(), scaled,
+                                                               want_doutput=want_doutput, want_params=want_params, want_input=want_input)
+            grads = (grads.to(torch.float32) / ctx.loss_scale).to(params.dtype) if grads is not None else None
+            dinput = (dinput / ctx.loss_scale).to(inputs.dtype) if dinput is not None else None
+        return None, None, ddoutput, dinput, grads, None, None
 
 
 class _TcnnModule(torch.nn.Module):
