@@ -157,6 +157,8 @@ int tcnnb_encoding_backward_backward_input(tcnnb_encoding* e, tcnnb_stream strea
  * padded outputs up to n_neurons). Parameters are CALLER-owned fp16 device arrays (16-byte aligned) in the reference's layout
  * (fully_fused_mlp.cu:635-672): W_0 [n_neurons][input_width], (n_hidden_layers - 1) x [n_neurons][n_neurons],
  * W_out [padded_output_width][n_neurons], row-major; input_width = n_input_dims rounded up to 16.
+ * Hidden activations: FullyFusedMLP's set (everything but Sine / SiLU); "CutlassMLP"/"MLP" also take Sine and SiLU, whose derivative
+ * needs the pre-activations: the forward pass then keeps both (cutlass_mlp.cu:162-209), see tcnnb_network_n_forward_activations.
  * Batches are multiples of 256. All work is stream-ordered; nothing synchronises. */
 typedef struct tcnnb_network tcnnb_network;
 int tcnnb_network_create(uint32_t n_input_dims, uint32_t n_output_dims, const char* network_json, tcnnb_network** out);
@@ -166,17 +168,24 @@ uint32_t tcnnb_network_input_width(const tcnnb_network* n);          /* n_input_
 uint32_t tcnnb_network_padded_output_width(const tcnnb_network* n);  /* network->padded_output_width() */
 uint32_t tcnnb_network_width(const tcnnb_network* n);
 uint32_t tcnnb_network_n_hidden_layers(const tcnnb_network* n);
-/* Network::initialize_params (fully_fused_mlp.cu:868-892): xavier uniform per matrix from pcg32{seed}; device fp32 [n_params]. */
+/* CutlassMLP::num_forward_activations(): the [n][n_neurons] hidden rows tcnnb_network_forward writes and tcnnb_network_backward reads
+ * -- n_hidden_layers, or 2 x n_hidden_layers for a Sine / SiLU hidden activation. */
+uint32_t tcnnb_network_n_forward_activations(const tcnnb_network* n);
+/* Network::initialize_params (fully_fused_mlp.cu:868-892): xavier uniform per matrix from pcg32{seed}; device fp32 [n_params]. A Sine
+ * network takes the SIREN initialisation (cutlass_mlp.cu:362-371): 30 / fan_in for W_0, sqrt(6 / fan_in) for the other matrices. */
 int tcnnb_network_initialize_params(tcnnb_network* n, uint64_t seed, float* params_full_precision_dev, float scale);
 /* network->inference_mixed_precision(stream, input, output) (object.h / network.h): input fp16 [n][n_input_dims] (n_input_dims
  * must be a multiple of 16), output fp16 [n][padded_output_width]. */
 int tcnnb_network_inference_mixed_precision(tcnnb_network* n, tcnnb_stream stream, uint32_t n_elements, const void* input_dev, void* output_dev, const void* params_dev);
 /* network->forward: the same, and the post-activation hidden layers fp16 [n_hidden_layers][n][n_neurons] are written out
- * (what the reference's ForwardContext holds, fully_fused_mlp.cu:841-854). output_dev may be null. */
+ * (what the reference's ForwardContext holds, fully_fused_mlp.cu:841-854). output_dev may be null. For a Sine / SiLU hidden
+ * activation hidden_dev is [2][n_hidden_layers][n][n_neurons]: the post-activations first, then the fp16 pre-activations z, with
+ * post = act(z) bit for bit (tcnnb_network_n_forward_activations() rows of [n][n_neurons] in all). */
 int tcnnb_network_forward(tcnnb_network* n, tcnnb_stream stream, uint32_t n_elements, const void* input_dev, void* output_dev, void* hidden_dev, const void* params_dev);
 /* network->backward (Network<T>::backward, fully_fused_mlp.cu:733-866) from what tcnnb_network_forward was given and wrote:
  * dL_doutput fp16 [n][padded_output_width] -> dL_dinput fp16 [n][n_input_dims] and dL_dparams fp16 [n_params] (OVERWRITTEN);
- * either may be null. output_dev is only read when the network has an output activation. Three kernels: the dgrad chain on
+ * either may be null. output_dev is only read when the network has an output activation; hidden_dev has tcnnb_network_forward's
+ * layout (Sine / SiLU: the derivative is taken at the pre-activations of its second half). Three kernels: the dgrad chain on
  * wgmma with the transposed weights read in place (mlp_fused.cu, BWD), the weight-gradient kernel (mlp_wgrad.cu), fp32 -> fp16. */
 int tcnnb_network_backward(tcnnb_network* n, tcnnb_stream stream, uint32_t n_elements, const void* input_dev, const void* output_dev, const void* hidden_dev,
                            const void* dL_doutput_dev, const void* params_dev, void* dL_dinput_dev, void* dL_dparams_dev);

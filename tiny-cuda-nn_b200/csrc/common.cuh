@@ -13,6 +13,9 @@ constexpr uint32_t TILE_M = 128;               // samples per MMA tile (two m64 
 
 // Same numeric values as the reference enums (common.h:133-164).
 enum Activation : uint32_t { ACT_RELU = 0, ACT_LEAKY_RELU = 1, ACT_SILU = 2, ACT_EXPONENTIAL = 3, ACT_SINE = 4, ACT_SIGMOID = 5, ACT_SQUAREPLUS = 6, ACT_SOFTPLUS = 7, ACT_TANH = 8, ACT_NONE = 9 };
+// Sine and SiLU: the derivative needs the pre-activation, so a network with them as hidden activation keeps both buffers per hidden
+// layer (CutlassMLP's m_can_fuse_activation, cutlass_mlp.cu:53, and num_forward_activations()).
+__host__ __device__ inline bool activation_needs_preact(uint32_t act) { return act == ACT_SINE || act == ACT_SILU; }
 enum GridType : uint32_t { GRID_HASH = 0, GRID_DENSE = 1, GRID_TILED = 2 };
 enum InterpolationType : uint32_t { INTERP_NEAREST = 0, INTERP_LINEAR = 1, INTERP_SMOOTHSTEP = 2 };
 enum LossType : uint32_t { LOSS_L2 = 0, LOSS_RELATIVE_L2 = 1, LOSS_L1 = 2, LOSS_RELATIVE_L1 = 3, LOSS_MAPE = 4, LOSS_SMAPE = 5, LOSS_RELATIVE_L2_LUMINANCE = 6, LOSS_CROSS_ENTROPY = 7, LOSS_VARIANCE_IS = 8 };

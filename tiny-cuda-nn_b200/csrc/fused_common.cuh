@@ -76,6 +76,38 @@ __device__ __forceinline__ __half act_bwd_h(uint32_t act, __half grad, __half fw
 	}
 }
 
+// ---- activations whose derivative needs the PRE-activation z (CutlassMLP only, cutlass_mlp.cu:53): Sine and SiLU. Kept apart from
+// act_fwd_h / act_bwd_h so that the kernels of the other activations do not carry their cases. Forward on the fp16 z as
+// warp_activation<__half> (common_device.h:131-153), so that the stored post-activation is a function of the stored z alone;
+// backward as warp_activation_backward_in<__half> (common_device.h:253-277): the factor rounded to fp16, the product in fp16.
+// Same fast-math lowering as the reference build (sinf / cosf / expf -> the hardware approximations).
+__device__ __forceinline__ float logistic_f(float x) { return 1.0f / (1.0f + expf(-x)); }
+
+__device__ __forceinline__ __half act_fwd_pre_h(uint32_t act, __half z) {
+	const float x = __half2float(z);
+	return __float2half_rn(act == ACT_SINE ? sinf(x) : x * logistic_f(x));
+}
+
+__device__ __forceinline__ __half act_bwd_pre_h(uint32_t act, __half grad, __half z) {
+	const float x = __half2float(z);
+	if (act == ACT_SINE) return __hmul(grad, __float2half_rn(cosf(x)));
+	const float l = logistic_f(x);
+	return __hmul(grad, __float2half_rn(l + x * (l * (1.0f - l))));  // SiLU
+}
+
+__device__ __forceinline__ uint32_t act_pre_pack(uint32_t act, uint32_t z_bits) {
+	const __half2 z = *reinterpret_cast<const __half2*>(&z_bits);
+	const __half2 y = __halves2half2(act_fwd_pre_h(act, __low2half(z)), act_fwd_pre_h(act, __high2half(z)));
+	return *reinterpret_cast<const uint32_t*>(&y);
+}
+
+__device__ __forceinline__ uint32_t act_bwd_pre_pack(uint32_t act, uint32_t lo_bits, uint32_t hi_bits, uint32_t z_bits) {
+	const __half2 g = __floats2half2_rn(__uint_as_float(lo_bits), __uint_as_float(hi_bits));
+	const __half2 z = *reinterpret_cast<const __half2*>(&z_bits);
+	const __half2 y = __halves2half2(act_bwd_pre_h(act, __low2half(g), __low2half(z)), act_bwd_pre_h(act, __high2half(g), __high2half(z)));
+	return *reinterpret_cast<const uint32_t*>(&y);
+}
+
 __device__ __forceinline__ uint32_t act_pack(uint32_t act, uint32_t lo_bits, uint32_t hi_bits) {
 	if (act == ACT_RELU) return relu_pack(lo_bits, hi_bits);  // packed fast path
 	const __half2 x = __floats2half2_rn(__uint_as_float(lo_bits), __uint_as_float(hi_bits));

@@ -52,10 +52,11 @@ struct MlpCfg {
 };
 
 struct MlpKernelParams {
-	MlpForwardParams p;
+	MlpChainParams p;
 	uint32_t n_stages;  // == n_steps when all matrices are resident
 	uint32_t resident;
 	uint32_t n_steps;   // MMAs chained per unit: n_hidden_layers + 1 (the backward chain without dL/d(input): n_hidden_layers)
+	__half* hidden_pre_out;  // MlpForwardParams::hidden_pre_out (PRE kernels only)
 };
 
 }  // namespace
@@ -76,11 +77,17 @@ struct MlpKernelParams {
 // -- the SAME bytes TMA delivered, W^T without a transposed copy --, the hidden epilogue multiplies by the activation's derivative
 // (from the forward pass's post-activation values in `hidden_in`) and writes g_l to `hidden_out` (for the weight-gradient kernel,
 // mlp_wgrad.cu), and what leaves is dL/d(input).
-template <uint32_t W, bool GENERIC_ACT, bool BWD>
+//
+// PRE = true (with GENERIC_ACT): the hidden activation is Sine or SiLU, whose derivative needs the PRE-activation z (the reference's
+// CutlassMLP keeps both buffers for them, cutlass_mlp.cu:162-209, 266-304). Forward: the hidden epilogue rounds z to fp16, stores it
+// to `hidden_pre_out` (when given) and applies the activation to that fp16 z. Backward: `hidden_in` holds the forward pass's z, and
+// the epilogue multiplies by act'(z).
+template <uint32_t W, bool GENERIC_ACT, bool BWD, bool PRE>
 __global__ void __launch_bounds__(MlpCfg<W>::THREADS, 1)
 mlp_forward_kernel(const MlpKernelParams kp, const __grid_constant__ CUtensorMap map_w0, const __grid_constant__ CUtensorMap map_wh, const __grid_constant__ CUtensorMap map_wo) {
 	using C = MlpCfg<W>;
-	const MlpForwardParams& p = kp.p;
+	static_assert(!PRE || GENERIC_ACT, "the pre-activation path is a generic-activation kernel");
+	const MlpChainParams& p = kp.p;
 	const uint32_t hid_act = GENERIC_ACT ? p.activation : (uint32_t)ACT_RELU;
 	const uint32_t out_act = BWD ? (uint32_t)ACT_NONE : (GENERIC_ACT ? p.output_activation : (uint32_t)ACT_NONE);
 	extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -194,8 +201,8 @@ mlp_forward_kernel(const MlpKernelParams kp, const __grid_constant__ CUtensorMap
 					if (lane == 0) mbar_arrive_plain(bar_w_free + 8 * stage);
 					continue;
 				}
-				// backward: the forward pass's activations of the layer this step lands on (hidden layer NH - 1 - l), fetched before
-				// the MMA so that the loads travel while it runs
+				// backward: the forward pass's activations (PRE: pre-activations) of the layer this step lands on (hidden layer NH - 1 - l),
+				// fetched before the MMA so that the loads travel while it runs
 				uint32_t fwd[BWD ? W / 4 : 1];
 				if (BWD && l < NH) {
 					const __half* hsrc = p.hidden_in + ((size_t)(NH - 1 - l) * p.batch_size + row0 + r0) * W + 2 * ft;
@@ -233,12 +240,22 @@ mlp_forward_kernel(const MlpKernelParams kp, const __grid_constant__ CUtensorMap
 					// hidden layer: fp32 accumulator -> (derivative of the) activation in fp16 -> the next product's A fragment; the rows
 					// also go to global memory when the caller keeps them (forward activations / backward g_l)
 					__half* keep = p.hidden_out ? p.hidden_out + ((size_t)(BWD ? NH - 1 - l : l) * p.batch_size + row0 + r0) * W + 2 * ft : nullptr;
+					__half* keep_pre = (PRE && !BWD && kp.hidden_pre_out) ? kp.hidden_pre_out + ((size_t)l * p.batch_size + row0 + r0) * W + 2 * ft : nullptr;
 #pragma unroll
 					for (uint32_t i = 0; i < W / 8; ++i) {
 #pragma unroll
 						for (uint32_t hi = 0; hi < 2; ++hi) {
 							const uint32_t lo_bits = __float_as_uint(acc[4 * i + 2 * hi]), hi_bits = __float_as_uint(acc[4 * i + 2 * hi + 1]);
-							const uint32_t v = BWD ? act_bwd_pack(hid_act, lo_bits, hi_bits, fwd[(2 * i + hi) % (BWD ? W / 4 : 1)]) : act_pack(hid_act, lo_bits, hi_bits);
+							uint32_t v;
+							if (PRE && BWD) {
+								v = act_bwd_pre_pack(hid_act, lo_bits, hi_bits, fwd[(2 * i + hi) % (BWD ? W / 4 : 1)]);
+							} else if (PRE) {
+								const uint32_t z = pack_half2(__uint_as_float(lo_bits), __uint_as_float(hi_bits));
+								if (keep_pre) *reinterpret_cast<uint32_t*>(keep_pre + hi * 8 * W + 8 * i) = z;
+								v = act_pre_pack(hid_act, z);
+							} else {
+								v = BWD ? act_bwd_pack(hid_act, lo_bits, hi_bits, fwd[(2 * i + hi) % (BWD ? W / 4 : 1)]) : act_pack(hid_act, lo_bits, hi_bits);
+							}
 							a[i / 2][(i & 1u) * 2 + hi] = v;
 							if (keep) *reinterpret_cast<uint32_t*>(keep + hi * 8 * W + 8 * i) = v;
 						}
@@ -277,13 +294,14 @@ uint32_t max_stages() {
 	return (uint32_t)((227u * 1024u - 1024u) / MlpCfg<W>::STAGE_BYTES) < MLPF_MAX_STAGES ? (uint32_t)((227u * 1024u - 1024u) / MlpCfg<W>::STAGE_BYTES) : MLPF_MAX_STAGES;
 }
 
-template <uint32_t W, bool GENERIC, bool BWD>
+template <uint32_t W, bool GENERIC, bool BWD, bool PRE = false>
 cudaError_t launch_impl(const MlpForwardParams& p, uint32_t n_sms, cudaStream_t stream) {
 	using C = MlpCfg<W>;
 	const uint32_t n_layers = p.n_hidden_layers + ((BWD && !p.output_fp16) ? 0 : 1);  // steps of the chain
 	MlpKernelParams kp{};
 	kp.p = p;
 	kp.n_steps = n_layers;
+	kp.hidden_pre_out = p.hidden_pre_out;
 	kp.resident = n_layers <= max_stages<W>() ? 1 : 0;
 	kp.n_stages = kp.resident ? n_layers : max_stages<W>();
 	CUtensorMap m0, mh, mo;
@@ -297,7 +315,7 @@ cudaError_t launch_impl(const MlpForwardParams& p, uint32_t n_sms, cudaStream_t 
 	}
 	w += (size_t)(p.n_hidden_layers - 1) * W * W;
 	if (!make_fp16_matrix_map(&mo, w, p.out_width, W, p.out_width)) return cudaErrorInvalidValue;
-	auto kernel = mlp_forward_kernel<W, GENERIC, BWD>;
+	auto kernel = mlp_forward_kernel<W, GENERIC, BWD, PRE>;
 	const size_t smem = (size_t)kp.n_stages * C::STAGE_BYTES + 8 * 2 * MLPF_MAX_STAGES;
 	cudaError_t err = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
 	if (err != cudaSuccess) return err;
@@ -307,6 +325,7 @@ cudaError_t launch_impl(const MlpForwardParams& p, uint32_t n_sms, cudaStream_t 
 
 template <uint32_t W>
 cudaError_t launch_width(const MlpForwardParams& p, uint32_t n_sms, cudaStream_t stream) {
+	if (activation_needs_preact(p.activation)) return p.backward ? launch_impl<W, true, true, true>(p, n_sms, stream) : launch_impl<W, true, false, true>(p, n_sms, stream);
 	if (p.backward) return p.activation != ACT_RELU ? launch_impl<W, true, true>(p, n_sms, stream) : launch_impl<W, false, true>(p, n_sms, stream);
 	const bool generic = p.activation != ACT_RELU || p.output_activation != ACT_NONE;
 	return generic ? launch_impl<W, true, false>(p, n_sms, stream) : launch_impl<W, false, false>(p, n_sms, stream);
@@ -339,6 +358,12 @@ bool mlp_forward_supported(const MlpForwardParams& p, const char** why) {
 	if (p.backward) {
 		if (!p.input_fp16 || !p.hidden_in || p.output_fp32) return fail("tcnn_b200: the backward chain needs dL/d(output) and the forward activations in fp16");
 		if (p.output_fp16 && p.in_width > (p.width < 32 ? 32u : p.width)) return fail("tcnn_b200: dL/d(input) of the stand-alone network covers inputs up to max(n_neurons, 32) wide");
+	}
+	if (activation_needs_preact(p.output_activation)) return fail("tcnn_b200: Sine / SiLU are hidden activations only; as output activation they have no derivative (warp_activation_backward)");
+	if (activation_needs_preact(p.activation)) {
+		if (!p.backward && p.hidden_out && !p.hidden_pre_out) return fail("tcnn_b200: Sine / SiLU keep the pre-activations for the backward pass: hidden_pre_out must be given with hidden_out");
+	} else if (p.hidden_pre_out) {
+		return fail("tcnn_b200: hidden_pre_out is only written for Sine / SiLU hidden activations");
 	}
 	if (p.input_fp32 && (p.n_input_dims == 0 || p.n_input_dims > p.in_width)) return fail("tcnn_b200: Identity encoding wider than the network input");
 	return true;

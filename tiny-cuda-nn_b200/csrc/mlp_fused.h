@@ -4,7 +4,8 @@
 
 namespace tcnnb {
 
-struct MlpForwardParams {
+// What the kernel reads from its parameter block (mlp_fused.cu, MlpKernelParams); the launch interface is MlpForwardParams below.
+struct MlpChainParams {
 	// network (fully_fused_mlp.cu:635-672): W_0 [width][in_width], (n_hidden_layers - 1) x [width][width], W_out [out_width][width],
 	// row-major fp16, contiguous in this order
 	uint32_t width;              // 16 / 32 / 64 / 128
@@ -28,13 +29,20 @@ struct MlpForwardParams {
 	__half* hidden_out;
 	// backward chain (Network<T>::backward's dgrad half, fully_fused_mlp.cu:733-800): with `backward` set,
 	//   input_fp16  = dL/d(output) [batch][out_width], already multiplied by the output activation's derivative,
-	//   hidden_in   = the forward pass's `hidden_out`,
+	//   hidden_in   = the forward pass's `hidden_out` (Sine / SiLU: its `hidden_pre_out`),
 	//   hidden_out  = g_l = dL/d(pre-activation of hidden layer l) [n_hidden_layers][batch][width] (may be null),
 	//   output_fp16 = dL/d(input) [batch][in_width] (may be null: the last step of the chain is then skipped).
 	uint32_t backward;
 	const __half* hidden_in;
 	// profiling only (tcnnb_network_debug_clocks): clock64 stamps [cta][consumer warpgroup (5 slots)][64 events][8], null in production
 	long long* dbg_clock;
+};
+
+struct MlpForwardParams : MlpChainParams {
+	// Sine / SiLU hidden activation only (activation_needs_preact): the fp16 PRE-activation rows z_l [n_hidden_layers][batch][width],
+	// required with hidden_out (the backward chain reads them as its `hidden_in`); hidden_out = act(hidden_pre_out) bit for bit.
+	// Kept out of MlpChainParams so that the parameter block of the other activations' kernels keeps its layout.
+	__half* hidden_pre_out;
 };
 
 // Maximum number of weight matrices that stay resident in shared memory for a width (more layers stream through a ring).
@@ -64,6 +72,7 @@ struct MlpBackwardArgs {
 	uint32_t batch_size;
 	const __half* input;          // [batch][in_width] forward input (weight gradients of the first matrix); may be null if dw_accum is
 	const __half* hidden;         // [n_hidden_layers][batch][width] forward activations
+	const __half* hidden_pre;     // [n_hidden_layers][batch][width] forward pre-activations; Sine / SiLU only (activation_needs_preact)
 	const __half* output;         // [batch][out_width] forward output; only read when output_activation != None
 	const __half* dL_doutput;     // [batch][out_width]
 	__half* grad_hidden;          // scratch [n_hidden_layers][batch][width]

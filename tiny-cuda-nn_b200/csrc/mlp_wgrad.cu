@@ -231,7 +231,7 @@ static void split_backward(const MlpBackwardArgs& a, MlpForwardParams& d, MlpWgr
 	d.input_fp16 = a.output_activation == ACT_NONE ? a.dL_doutput : a.grad_output;
 	d.output_fp16 = a.dL_dinput;
 	d.hidden_out = a.grad_hidden;
-	d.hidden_in = a.hidden;
+	d.hidden_in = activation_needs_preact(a.activation) ? a.hidden_pre : a.hidden;  // Sine / SiLU: the derivative reads z
 	d.backward = 1;
 	w = MlpWgradParams{};
 	w.width = a.width;
@@ -252,6 +252,10 @@ bool mlp_backward_supported(const MlpBackwardArgs& a, const char** why) {
 	split_backward(a, d, w);
 	if (!d.input_fp16) d.input_fp16 = (const __half*)16;  // probing a shape: only null-ness matters
 	if (!d.hidden_in) d.hidden_in = (const __half*)16;
+	if (activation_needs_preact(a.activation) && a.hidden && !a.hidden_pre) {
+		if (why) *why = "tcnn_b200: the backward pass of a Sine / SiLU network needs the forward pass's pre-activations (hidden_pre)";
+		return false;
+	}
 	return mlp_forward_supported(d, why) && mlp_wgrad_supported(w, why);
 }
 
@@ -259,6 +263,7 @@ cudaError_t launch_mlp_backward(const MlpBackwardArgs& a, uint32_t n_sms, cudaSt
 	MlpForwardParams d;
 	MlpWgradParams w;
 	split_backward(a, d, w);
+	if (!d.hidden_in || (activation_needs_preact(a.activation) && a.dw_accum && !a.hidden)) return cudaErrorInvalidValue;
 	uint32_t launches = 0;
 	cudaError_t err = cudaSuccess;
 	if (a.output_activation != ACT_NONE) {

@@ -254,6 +254,7 @@ static const char* general_path_unsupported(const Model& m) {
 static const char* fused_kernel_unsupported(const EncodingPlan& plan, const MlpConfig& mlp, uint32_t n_in) {
 	const GridConfig* grid = single_encoding(plan, FEAT_GRID) ? &plan.grids[0]->cfg : nullptr;
 	if (!grid && !single_encoding(plan, FEAT_IDENTITY)) return "an encoding other than one grid / Identity";
+	if (activation_needs_preact(mlp.activation)) return "an activation that needs stored pre-activations (Sine / SiLU)";
 	if (mlp.width > 64) return "n_neurons > 64";
 	if (mlp.n_hidden_layers > 6) return "n_hidden_layers > 6";
 	if (mlp.padded_out_width != 16) return "more than 16 outputs";
@@ -530,8 +531,12 @@ static void general_forward(Model& m, cudaStream_t stream, uint32_t batch, const
 	p.output_fp16 = out_fp16;
 	p.output_fp32 = out_fp32;
 	if (keep_hidden) {
-		grow(m.g_hidden, (size_t)mlp.n_hidden_layers * batch * mlp.width);
+		// Sine / SiLU: the pre-activations follow the post-activations in the same buffer
+		const size_t n_hidden = (size_t)mlp.n_hidden_layers * batch * mlp.width;
+		const bool pre = activation_needs_preact(mlp.activation);
+		grow(m.g_hidden, pre ? 2 * n_hidden : n_hidden);
 		p.hidden_out = m.g_hidden.ptr;
+		p.hidden_pre_out = pre ? m.g_hidden.ptr + n_hidden : nullptr;
 	}
 	const char* why = nullptr;
 	if (!mlp_forward_supported(p, &why)) throw std::runtime_error(why);
@@ -569,6 +574,7 @@ static void general_backward_pass(Model& m, cudaStream_t stream, uint32_t batch,
 	a.batch_size = batch;
 	a.input = m.g_enc.ptr;
 	a.hidden = m.g_hidden.ptr;
+	if (activation_needs_preact(mlp.activation)) a.hidden_pre = m.g_hidden.ptr + (size_t)mlp.n_hidden_layers * batch * mlp.width;
 	a.output = out;
 	if (ext_dL_doutput) {  // Module::backward: the caller's dL/d(output) still has to pass the output activation (fully_fused_mlp.cu:755-762)
 		a.output_activation = mlp.output_activation;

@@ -3,7 +3,10 @@
 // Mirrors, for FullyFusedMLP on its own,
 //   src/network.cu:51-141         create_network<T>(json): "otype", "n_neurons", "n_hidden_layers", "activation", "output_activation"
 //   fully_fused_mlp.cu:635-672    parameter layout: W_0 [width][in], (n_hidden - 1) x [width][width], W_out [padded_out][width]
-//   fully_fused_mlp.cu:868-892    initialize_params: xavier uniform per matrix, one pcg32 stream (gpu_matrix.h:292-306)
+//   fully_fused_mlp.cu:868-892    initialize_params: xavier uniform per matrix, one pcg32 stream (gpu_matrix.h:292-306); SIREN for a
+//                                 Sine CutlassMLP (cutlass_mlp.cu:362-371)
+//   cutlass_mlp.cu:162-209        Sine / SiLU (CutlassMLP): the forward pass keeps pre- and post-activations, num_forward_activations()
+//                                 = 2 x n_hidden_layers (tcnnb_network_n_forward_activations)
 //   object.h:214-282 / network.h  inference_mixed_precision (fp16 in, fp16 out) and inference (fp32 in, fp32 out)
 //   src/cpp_api.cu:160-162        cpp::create_network = the network behind an Identity encoding (encodings/identity.h:46-67)
 // Parameters are CALLER-owned fp16 device arrays, as in the module tier. No fallback: an unsupported shape is an error.
@@ -44,6 +47,16 @@ static void build_network(Network& n, uint32_t n_in, uint32_t n_out, const json:
 	probe.input_fp16 = (const __half*)16;
 	const char* why = nullptr;
 	if (!mlp_forward_supported(probe, &why)) throw std::runtime_error(why);
+}
+
+// Hidden rows per hidden layer the forward pass keeps for the backward pass (CutlassMLP::num_forward_activations()): the post-
+// activations, and for Sine / SiLU the pre-activations after them.
+static uint32_t n_forward_activations(const MlpConfig& c) { return activation_needs_preact(c.activation) ? 2 * c.n_hidden_layers : c.n_hidden_layers; }
+
+// The pre-activation half of a `hidden` buffer [2][n_hidden_layers][batch][width] (Sine / SiLU), else null.
+template <typename T>
+static T* hidden_pre_of(const MlpConfig& c, T* hidden, uint32_t batch) {
+	return (hidden && activation_needs_preact(c.activation)) ? hidden + (size_t)c.n_hidden_layers * batch * c.width : nullptr;
 }
 
 static MlpForwardParams make_params(const Network& n, uint32_t batch, const void* params) {
@@ -92,6 +105,7 @@ static void network_backward(Network& n, cudaStream_t stream, uint32_t batch, co
 	a.batch_size = batch;
 	a.input = input;
 	a.hidden = hidden;
+	a.hidden_pre = hidden_pre_of(n.cfg, hidden, batch);
 	a.output = output;
 	a.dL_doutput = dL_doutput;
 	a.dL_dinput = dL_dinput;
@@ -145,6 +159,7 @@ uint32_t tcnnb_network_input_width(const tcnnb_network* n) { return n->impl.cfg.
 uint32_t tcnnb_network_padded_output_width(const tcnnb_network* n) { return n->impl.cfg.padded_out_width; }
 uint32_t tcnnb_network_width(const tcnnb_network* n) { return n->impl.cfg.width; }
 uint32_t tcnnb_network_n_hidden_layers(const tcnnb_network* n) { return n->impl.cfg.n_hidden_layers; }
+uint32_t tcnnb_network_n_forward_activations(const tcnnb_network* n) { return n_forward_activations(n->impl.cfg); }
 
 int tcnnb_network_debug_clocks(tcnnb_network* n, void* clocks_dev) {
 	TCNNB_API_BEGIN
@@ -185,6 +200,7 @@ int tcnnb_network_forward(tcnnb_network* n, tcnnb_stream stream, uint32_t n_elem
 	p.input_fp16 = (const __half*)input_dev;
 	p.output_fp16 = (__half*)output_dev;
 	p.hidden_out = (__half*)hidden_dev;
+	p.hidden_pre_out = hidden_pre_of(net.cfg, (__half*)hidden_dev, n_elements);
 	launch(net, p, (cudaStream_t)stream);
 	TCNNB_API_END
 }
@@ -214,13 +230,14 @@ int tcnnb_network_module_backward(tcnnb_network* n, tcnnb_stream stream_, uint32
 	if (((uintptr_t)dL_doutput_dev | (uintptr_t)dL_dparams_dev) % 16 != 0) throw std::runtime_error("network: dL_doutput / dL_dparams must be 16-byte aligned.");
 	MlpForwardParams p = make_params(net, n_elements, params_dev);
 	grow(net.enc_input, (size_t)n_elements * net.cfg.in_width);
-	grow(net.hidden, (size_t)net.cfg.n_hidden_layers * n_elements * net.cfg.width);
+	grow(net.hidden, (size_t)n_forward_activations(net.cfg) * n_elements * net.cfg.width);
 	grow(net.output, (size_t)n_elements * net.cfg.padded_out_width);
 	TCNNB_CUDA_CHECK(launch_identity_encode(stream, n_elements, net.n_input_dims, net.cfg.in_width, 1.0f, 0.0f, input_dev, net.enc_input.ptr));
 	++g_kernel_launches;
 	p.input_fp16 = net.enc_input.ptr;
 	p.output_fp16 = net.output.ptr;
 	p.hidden_out = net.hidden.ptr;
+	p.hidden_pre_out = hidden_pre_of(net.cfg, net.hidden.ptr, n_elements);
 	launch(net, p, stream);
 	__half* dL_denc = nullptr;
 	if (dL_dinput_dev) {

@@ -42,9 +42,12 @@ inline MlpConfig parse_network(const json::Value& net, uint32_t in_width, uint32
 		throw std::runtime_error("FullyFusedMLP only supports 16, 32, 64, and 128 neurons, but got " + std::to_string(c.width) + ". Use CutlassMLP instead if this is a requirement.");
 	}
 	if (c.n_hidden_layers < 1) throw std::runtime_error("FullyFusedMLP requires at least 1 hidden layer (3 layers in total).");
-	for (uint32_t act : {c.activation, c.output_activation}) {
-		// FullyFusedMLP's activation set (fully_fused_mlp.cu:689-699): Sine and SiLU need stored pre-activations
-		if (act == ACT_SINE || act == ACT_SILU) throw std::runtime_error("Unsupported activation.");
+	// Sine and SiLU need stored pre-activations: FullyFusedMLP rejects them (fully_fused_mlp.cu:689-699); CutlassMLP keeps them
+	// (cutlass_mlp.cu:53, 162-209) as the hidden activation. As output activation they have no derivative in the reference
+	// (warp_activation_backward leaves the gradient unwritten, common_device.h:375-390), so both otypes reject them there.
+	if (fully_fused && activation_needs_preact(c.activation)) throw std::runtime_error("Unsupported activation.");
+	if (activation_needs_preact(c.output_activation)) {
+		throw std::runtime_error("Unsupported activation. Sine / SiLU are not supported as output_activation: they have no output-activation derivative (CutlassMLP accepts them as the hidden activation).");
 	}
 	c.in_width = in_width;
 	c.out_width = n_out;
@@ -53,7 +56,10 @@ inline MlpConfig parse_network(const json::Value& net, uint32_t in_width, uint32
 	return c;
 }
 
-// Xavier uniform per matrix on the host, sequential draws from `rng` (fully_fused_mlp.cu:868-892, gpu_matrix.h:292-306).
+// Xavier uniform per matrix on the host, sequential draws from `rng` (fully_fused_mlp.cu:868-892, gpu_matrix.h:292-306). A Sine
+// network takes the SIREN initialisation instead (cutlass_mlp.cu:362-371): bound scale * 30 / fan_in for the first matrix
+// (initialize_siren_uniform_first, gpu_matrix.h:360-377), scale * sqrt(6 / fan_in) for the others, the output matrix included
+// (initialize_siren_uniform, gpu_matrix.h:343-358); same draw order and expression per element.
 // `dst`: DEVICE fp32 array of c.n_params elements.
 inline void init_mlp_params(const MlpConfig& c, HostPcg32& rng, float* dst, float scale) {
 	std::vector<float> w(c.n_params);
@@ -62,8 +68,12 @@ inline void init_mlp_params(const MlpConfig& c, HostPcg32& rng, float* dst, floa
 	for (uint32_t i = 0; i + 1 < c.n_hidden_layers; ++i) mats.emplace_back(c.width, c.width);
 	mats.emplace_back(c.padded_out_width, c.width);
 	size_t pos = 0;
-	for (auto& rc : mats) {
-		const float bound = scale * std::sqrt(6.0f / (float)(rc.second + rc.first));
+	for (size_t m = 0; m < mats.size(); ++m) {
+		const auto& rc = mats[m];
+		float bound = scale;
+		if (c.activation != ACT_SINE) bound *= std::sqrt(6.0f / (float)(rc.second + rc.first));
+		else if (m == 0) bound *= 30.0f / (float)rc.second;
+		else bound *= std::sqrt(6.0f / (float)rc.second);
 		for (size_t i = 0; i < (size_t)rc.first * rc.second; ++i) w[pos++] = rng.next_float() * 2.0f * bound - bound;
 	}
 	TCNNB_CUDA_CHECK(cudaMemcpy(dst, w.data(), sizeof(float) * w.size(), cudaMemcpyHostToDevice));

@@ -87,6 +87,7 @@ ABI = [
     ("tcnnb_network_padded_output_width", _u32, [_vp]),
     ("tcnnb_network_width", _u32, [_vp]),
     ("tcnnb_network_n_hidden_layers", _u32, [_vp]),
+    ("tcnnb_network_n_forward_activations", _u32, [_vp]),
     ("tcnnb_network_initialize_params", _int, [_vp, _u64, _vp, ctypes.c_float]),
     ("tcnnb_network_inference_mixed_precision", _int, [_vp, _vp, _u32, _vp, _vp, _vp]),
     ("tcnnb_network_forward", _int, [_vp, _vp, _u32, _vp, _vp, _vp, _vp]),
@@ -569,6 +570,8 @@ class Network:
         self.padded_output_width = lib.tcnnb_network_padded_output_width(h)
         self.width = lib.tcnnb_network_width(h)
         self.n_hidden_layers = lib.tcnnb_network_n_hidden_layers(h)
+        # hidden rows the forward pass keeps: n_hidden_layers, twice that for Sine / SiLU (post-activations, then pre-activations)
+        self.n_forward_activations = lib.tcnnb_network_n_forward_activations(h)
 
     def initial_params(self, seed=1337, scale=1.0):
         import torch
@@ -586,12 +589,13 @@ class Network:
         return out
 
     def forward(self, x16, params16, stream=None):
-        """-> (output fp16 [n][padded_out], hidden fp16 [n_hidden_layers][n][width])"""
+        """-> (output fp16 [n][padded_out], hidden fp16 [n_forward_activations][n][width]): the post-activations of every hidden layer,
+        followed for Sine / SiLU by the pre-activations."""
         import torch
 
         n = x16.shape[0]
         out = torch.empty(n, self.padded_output_width, dtype=torch.float16, device=x16.device)
-        hidden = torch.empty(self.n_hidden_layers, n, self.width, dtype=torch.float16, device=x16.device)
+        hidden = torch.empty(self.n_forward_activations, n, self.width, dtype=torch.float16, device=x16.device)
         _check(load().tcnnb_network_forward(self._h, _stream_handle(stream), n, x16.data_ptr(), out.data_ptr(), hidden.data_ptr(), params16.data_ptr()))
         return out, hidden
 
