@@ -3,6 +3,9 @@
 --reference the same points on the unmodified reference (oracle/_ref/ref_harness mlpbench: fully_fused_jit, fully_fused, cutlass).
 
     python scripts/bench_mlp.py [--widths 16,32,64,128] [--hidden 2,4,8] [--batches 16384,...] [--iters N] [--reference]
+                                [--otype FullyFusedMLP | CutlassMLP]
+
+--otype CutlassMLP also runs 256 neurons (--widths 256); --reference then times the reference's own CutlassMLP beside each point.
 
 Roofline per point (SURVEY.md section 8d): FLOPs/sample = 2 (in*w + (h-1) w^2 + w*out); bytes/sample = 2 (in + out). The line carries
 the achieved TFLOP/s against the measured bf16 tensor peak and the achieved GB/s against the measured HBM copy peak, whichever
@@ -33,6 +36,7 @@ def main():
     ap.add_argument("--batches", default="16384,262144,4194304")
     ap.add_argument("--iters", type=int, default=0)
     ap.add_argument("--reference", action="store_true")
+    ap.add_argument("--otype", default="FullyFusedMLP", choices=["FullyFusedMLP", "CutlassMLP"])
     args = ap.parse_args()
     import torch
 
@@ -42,7 +46,7 @@ def main():
     harness = os.path.join(ROOT, "oracle", "_ref", "ref_harness")
     for width in [int(v) for v in args.widths.split(",")]:
         for hidden in [int(v) for v in args.hidden.split(",")]:
-            net = tcnn_b200.Network(width, width, {"otype": "FullyFusedMLP", "n_neurons": width, "n_hidden_layers": hidden, "activation": "ReLU", "output_activation": "None"})
+            net = tcnn_b200.Network(width, width, {"otype": args.otype, "n_neurons": width, "n_hidden_layers": hidden, "activation": "ReLU", "output_activation": "None"})
             p16 = net.initial_params(1337).to(torch.float16).contiguous()
             for B in [int(v) for v in args.batches.split(",")]:
                 x = torch.rand(B, width, device="cuda").to(torch.float16).contiguous()
@@ -59,12 +63,13 @@ def main():
                 ms = e0.elapsed_time(e1) / iters
                 flops = 2.0 * (width * width * (hidden + 1)) * B
                 byts = 2.0 * (width + width) * B
-                line = {"impl": "tcnn_b200", "mode": "mlp_inference", "width": width, "n_hidden_layers": hidden, "batch": B, "iters": iters, "ms_per_batch": ms,
+                line = {"impl": "tcnn_b200", "mode": "mlp_inference", "otype": args.otype, "width": width, "n_hidden_layers": hidden, "batch": B, "iters": iters, "ms_per_batch": ms,
                         "samples_per_s": B / (ms * 1e-3), "tflops": flops / (ms * 1e-3) / 1e12, "gbs": byts / (ms * 1e-3) / 1e9,
                         "tensor_frac": flops / (ms * 1e-3) / 1e12 / tensor, "hbm_frac": byts / (ms * 1e-3) / 1e9 / hbm, "peaks": kind}
                 if args.reference and os.path.exists(harness):
                     ref = {}
-                    for name, otype, jit in (("fully_fused_jit", "FullyFusedMLP", 1), ("fully_fused", "FullyFusedMLP", 0), ("cutlass", "CutlassMLP", 0)):
+                    modes = (("fully_fused_jit", "FullyFusedMLP", 1), ("fully_fused", "FullyFusedMLP", 0), ("cutlass", "CutlassMLP", 0))
+                    for name, otype, jit in modes if args.otype == "FullyFusedMLP" else modes[2:]:
                         cmd = [harness, "mlpbench", otype, str(width), str(hidden), str(width), str(width), str(B), str(iters), str(max(3, iters // 10)), str(jit)]
                         try:
                             out = subprocess.run(cmd, capture_output=True, text=True, timeout=600, cwd=ROOT)

@@ -2,7 +2,9 @@
 """Cost of the pre-activation path: HashGrid + CutlassMLP training steps (the general path) with ReLU against Sine and SiLU, whose
 kernels also write the fp16 pre-activations in the forward pass and read them in the backward chain.
 
-    python scripts/bench_preact.py [--batch-log2 18] [--steps 50] [--rounds 5]
+    python scripts/bench_preact.py [--batch-log2 18] [--steps 50] [--rounds 5] [--networks 64x2,128x4]
+
+--networks takes n_neurons x n_hidden_layers pairs, e.g. 256x3,256x8 for SIREN / neural-SDF sized networks.
 
 The activations are timed in alternation (one block of --steps steps per activation and round, CUDA events), so that clock and
 thermal drift hits all of them alike; the median and range over the rounds are printed, one JSON line per configuration."""
@@ -20,7 +22,7 @@ import torch  # noqa: E402
 import tcnn_b200  # noqa: E402
 
 ENCODING = {"otype": "HashGrid", "n_levels": 16, "n_features_per_level": 2, "log2_hashmap_size": 19, "base_resolution": 16, "per_level_scale": 1.5}
-NETWORKS = [(64, 2), (128, 4)]
+NETWORKS = "64x2,128x4"
 # "ReLU*": ReLU forced onto the general path (a 64-wide ReLU network otherwise takes the fused training kernel), the like-for-like
 # baseline of the Sine / SiLU steps
 ACTIVATIONS = ["ReLU", "ReLU*", "Sine", "SiLU"]
@@ -32,12 +34,13 @@ def main():
     ap.add_argument("--steps", type=int, default=50)
     ap.add_argument("--warmup", type=int, default=10)
     ap.add_argument("--rounds", type=int, default=5)
+    ap.add_argument("--networks", default=NETWORKS)
     args = ap.parse_args()
     B = 1 << args.batch_log2
     g = torch.Generator(device="cuda").manual_seed(0)
     x = torch.rand(B, 3, device="cuda", generator=g)
     y = torch.rand(B, 3, device="cuda", generator=g)
-    for width, nh in NETWORKS:
+    for width, nh in [tuple(int(v) for v in n.split("x")) for n in args.networks.split(",")]:
         models = {}
         for act in ACTIVATIONS:
             cfg = {"loss": {"otype": "L2"}, "optimizer": {"otype": "Adam", "learning_rate": 1e-3}, "encoding": ENCODING,

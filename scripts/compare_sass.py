@@ -6,7 +6,10 @@ untouched:
 
 Instruction text is compared with addresses and column padding removed. A kernel template that gained a trailing `bool` parameter
 (`mlp_forward_kernel<W, GENERIC_ACT, BWD, PRE>`) is matched to its old name when the new parameter is false. Exit code 1 if any old
-kernel is missing or differs."""
+kernel is missing or differs.
+
+Build both objects from the same source path (e.g. stash the change, build, unstash, build): kernels in an anonymous namespace
+carry a hash of the path in their mangled names, so objects built from two checkouts report every such kernel MISSING."""
 import re
 import subprocess
 import sys
@@ -31,13 +34,14 @@ def old_name(name):
 
 def main():
     old, new = functions(sys.argv[1]), functions(sys.argv[2])
-    by_old_name = {old_name(k): v for k, v in new.items()}
+    # a kernel whose name is unchanged is matched by that name first (old_name would strip its own trailing false parameter)
+    by_old_name = {**{old_name(k): v for k, v in new.items()}, **new}
     bad = 0
     for name, sass in old.items():
         if by_old_name.get(name) != sass:
             print("DIFFERENT" if name in by_old_name else "MISSING", name)
             bad += 1
-    added = [k for k in new if old_name(k) not in old]
+    added = [k for k in new if k not in old and old_name(k) not in old]
     print(f"{len(old) - bad} of {len(old)} kernels identical; {len(added)} new: {' '.join(added)}")
     sys.exit(1 if bad else 0)
 

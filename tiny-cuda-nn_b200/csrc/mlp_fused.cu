@@ -286,6 +286,239 @@ mlp_forward_kernel(const MlpKernelParams kp, const __grid_constant__ CUtensorMap
 	pdl_launch_dependents();
 }
 
+// 256 neurons (CutlassMLP): the same machine, with every product split into two N = 128 halves. Unsplit, a thread would hold the
+// K = 256 A fragment (64 registers), an N = 256 accumulator (128) and, backward, the prefetched forward rows (64) -- 256 registers before
+// addresses, more than a thread can have. Split:
+//   * half 0's epilogue packs into `a_lo`, a separate 32-register half of the next A fragment (half 1's MMAs still read all of `a`);
+//     half 1's epilogue writes k-steps 8 .. 15 of `a` once its MMAs are complete, then `a_lo` moves into k-steps 0 .. 7;
+//   * backward, the forward pass's rows are fetched per half (32 registers);
+//   * every half is a weight stage of its own, 64 KB: forward [128 rows][256 K] (four K-major [128][64] boxes), backward two
+//     MN-major [256 K rows][64 N] boxes. Three stages form a ring (a matrix is 128 KB: none stays resident);
+//   * a last product at most 128 wide (the network output forward, dL/d(input) backward) is one half.
+struct Mlp256 {
+	static constexpr uint32_t W = 256;
+	static constexpr uint32_t HALF = 128;
+	// ONE consumer warpgroup: the SM's register file is four 16 384-register quarters, and a warp lives in one of them; with two
+	// consumer warpgroups and the producer warp one quarter holds three warps, which caps every thread at 168 registers -- less than
+	// a 256-wide chain needs without spills. Four consumer warps and the producer warp leave up to 255.
+	static constexpr uint32_t WGS = 1;
+	static constexpr uint32_t THREADS = WGS * 128 + 32;
+	static constexpr uint32_t STAGE_BYTES = 65536;
+	static constexpr uint32_t STAGES = 3;
+	static constexpr uint32_t FWD_BOX_BYTES = HALF * 128;  // [128 rows][64 K]
+	static constexpr uint32_t BWD_BOX_BYTES = W * 128;     // [256 K rows][64 N]
+};
+
+template <bool GENERIC_ACT, bool BWD, bool PRE>
+__global__ void __launch_bounds__(Mlp256::THREADS, 1)
+mlp_forward256_kernel(const MlpKernelParams kp, const __grid_constant__ CUtensorMap map_w0, const __grid_constant__ CUtensorMap map_wh, const __grid_constant__ CUtensorMap map_wo) {
+	using C = Mlp256;
+	constexpr uint32_t W = C::W;
+	static_assert(!PRE || GENERIC_ACT, "the pre-activation path is a generic-activation kernel");
+	const MlpChainParams& p = kp.p;
+	const uint32_t hid_act = GENERIC_ACT ? p.activation : (uint32_t)ACT_RELU;
+	const uint32_t out_act = BWD ? (uint32_t)ACT_NONE : (GENERIC_ACT ? p.output_activation : (uint32_t)ACT_NONE);
+	extern __shared__ __align__(1024) uint8_t smem_raw[];
+	const uint32_t tid = threadIdx.x;
+	const uint32_t warp = __shfl_sync(0xFFFFFFFFu, tid >> 5, 0);
+	const uint32_t lane = tid & 31u;
+	const uint32_t NH = p.n_hidden_layers, n_layers = kp.n_steps;
+	const uint32_t in_w = p.in_width, out_w = p.out_width;
+	const uint32_t first_w = BWD ? out_w : in_w;
+	const uint32_t last_w = BWD ? in_w : out_w;
+	// Every step walks two half-stages. A last product at most 128 wide (the network output forward, dL/d(input) backward) needs
+	// only half 0: half 1's stage then carries no load and no MMA (its barrier is only arrived at), so that the wgmma code has no
+	// data-dependent branch around it.
+	auto one_half = [&](uint32_t l) { return l == NH && last_w <= C::HALF; };
+
+	const uint32_t smem_base = smem_u32(smem_raw);
+	if (smem_base & 1023u) __trap();
+	const uint32_t s_stage0 = smem_base;
+	const uint32_t bar_w_full = s_stage0 + C::STAGES * C::STAGE_BYTES;
+	const uint32_t bar_w_free = bar_w_full + 8 * MLPF_MAX_STAGES;
+
+	if (tid == 0) {
+		for (uint32_t i = 0; i < C::STAGES; ++i) {
+			mbar_init(bar_w_full + 8 * i, 1);
+			mbar_init(bar_w_free + 8 * i, C::WGS * 4);
+		}
+		fence_mbar_init();
+	}
+	if (warp == C::WGS * 4 && lane == 0) {
+		tma_prefetch_desc(&map_w0);
+		tma_prefetch_desc(&map_wh);
+		tma_prefetch_desc(&map_wo);
+	}
+	__syncthreads();
+	pdl_wait();
+
+	const uint32_t n_units = p.batch_size / UNIT_M;
+	const uint32_t n_my = blockIdx.x < n_units ? (n_units - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
+	const uint32_t n_rounds = (n_my + C::WGS - 1) / C::WGS;
+
+	if (warp == C::WGS * 4) {
+		// =============================================================================== TMA producer: half-matrices -> the stage ring
+		if (lane == 0) {
+			uint32_t g = 0;
+			for (uint32_t r = 0; r < (n_my ? n_rounds : 0u); ++r) {
+				for (uint32_t step = 0; step < n_layers; ++step) {
+					const uint32_t l = BWD ? NH - step : step;  // matrix of this step
+					const CUtensorMap* map = l == 0 ? &map_w0 : (l < NH ? &map_wh : &map_wo);
+					const int32_t row = l == 0 || l == NH ? 0 : (int32_t)((l - 1) * W);
+					for (uint32_t h = 0; h < 2; ++h, ++g) {
+						const uint32_t stage = g % C::STAGES;
+						if (g >= C::STAGES) mbar_wait(bar_w_free + 8 * stage, ((g / C::STAGES) - 1u) & 1u);
+						const uint32_t dst = s_stage0 + stage * C::STAGE_BYTES;
+						const uint32_t full = bar_w_full + 8 * stage;
+						if (h == 1 && one_half(step)) {
+							mbar_arrive_plain(full);
+						} else if (BWD) {
+							// K = the matrix's rows (all of them, one box), N = its columns 128 h ..: two 64-column boxes
+							mbar_arrive_expect_tx(full, 2 * C::BWD_BOX_BYTES);
+							for (uint32_t b = 0; b < 2; ++b) tma_load_2d(dst + b * C::BWD_BOX_BYTES, map, full, (int32_t)((2 * h + b) * 64), row);
+						} else {
+							// N = the matrix's rows 128 h .., K = its columns: one [128][64] box per 64 K-columns
+							const uint32_t kb = l == 0 ? (in_w + 63) / 64 : 4u;
+							mbar_arrive_expect_tx(full, kb * C::FWD_BOX_BYTES);
+							for (uint32_t b = 0; b < kb; ++b) tma_load_2d(dst + b * C::FWD_BOX_BYTES, map, full, (int32_t)(b * 64), row + (int32_t)(h * C::HALF));
+						}
+					}
+				}
+			}
+		}
+	} else {
+		// =============================================================================== consumer warpgroup s
+		const uint32_t s = warp / 4, wq = warp & 3u;
+		const uint32_t fq = lane >> 2, ft = lane & 3u;
+		const uint32_t r0 = wq * 16 + fq;
+		const bool stamp = wq == 0 && lane == 0;
+		uint32_t a[W / 16][4];          // A fragment of the next product
+		uint32_t a_lo[W / 32][4];       // half 0's epilogue: k-steps 0 .. 7 of the product after next
+		float acc[C::HALF / 2];
+		uint32_t g = 0;
+		for (uint32_t r = 0; r < n_rounds; ++r) {
+			const uint32_t j = r * C::WGS + s;
+			const bool real = j < n_my;
+			const size_t row0 = (size_t)(blockIdx.x + j * gridDim.x) * UNIT_M;
+			if (real) {
+#pragma unroll
+				for (uint32_t kk = 0; kk < W / 16; ++kk) {
+#pragma unroll
+					for (uint32_t q = 0; q < 4; ++q) {
+						const size_t rr = row0 + r0 + (q & 1u) * 8;
+						const uint32_t c = kk * 16 + (q >> 1) * 8 + 2 * ft;
+						uint32_t v = 0;
+						if (c < first_w) {
+							if (p.input_fp16) {
+								v = __ldg(reinterpret_cast<const uint32_t*>(p.input_fp16 + rr * first_w + c));
+							} else {
+								const float* src = p.input_fp32 + rr * p.n_input_dims;
+								const float lo = c < p.n_input_dims ? __ldg(src + c) : 1.0f;
+								const float hi = c + 1 < p.n_input_dims ? __ldg(src + c + 1) : 1.0f;
+								v = pack_half2(lo, hi);
+							}
+						}
+						a[kk][q] = v;
+					}
+				}
+			}
+			for (uint32_t l = 0; l < n_layers; ++l) {
+				const uint32_t ksteps = (l == 0 ? first_w : W) / 16;
+				const bool skip_half1 = one_half(l);
+#pragma unroll
+				for (uint32_t h = 0; h < 2; ++h) {
+					const uint32_t stage = g % C::STAGES;
+					if (stamp) MLPF_STAMP(s, g, 0);
+					mbar_wait(bar_w_full + 8 * stage, (g / C::STAGES) & 1u);
+					if (stamp) MLPF_STAMP(s, g, 1);
+					++g;
+					if (!real) {
+						__syncwarp();
+						if (lane == 0) mbar_arrive_plain(bar_w_free + 8 * stage);
+						continue;
+					}
+					uint32_t fwd[BWD ? C::HALF / 4 : 1];
+					if (BWD && l < NH) {
+						const __half* hsrc = p.hidden_in + ((size_t)(NH - 1 - l) * p.batch_size + row0 + r0) * W + h * C::HALF + 2 * ft;
+#pragma unroll
+						for (uint32_t i = 0; i < C::HALF / 8; ++i) {
+							fwd[(2 * i) % (BWD ? C::HALF / 4 : 1)] = __ldg(reinterpret_cast<const uint32_t*>(hsrc + 8 * i));
+							fwd[(2 * i + 1) % (BWD ? C::HALF / 4 : 1)] = __ldg(reinterpret_cast<const uint32_t*>(hsrc + 8 * W + 8 * i));
+						}
+					}
+					const uint32_t b_smem = s_stage0 + stage * C::STAGE_BYTES;
+					wgmma_fence();
+#pragma unroll
+					for (uint32_t kk = 0; kk < W / 16; ++kk) {
+						if (kk < ksteps && !(h == 1 && skip_half1)) {
+							const uint64_t b_desc = BWD ? wgmma_desc_sw128(b_smem + kk * 2048u, C::BWD_BOX_BYTES, 1024u)
+							                            : wgmma_desc_sw128(b_smem + (kk >> 2) * C::FWD_BOX_BYTES + (kk & 3u) * 32u, 16u, 1024u);
+							Wgmma<C::HALF>::template rs<BWD ? 1 : 0>(acc, a[kk], b_desc, kk > 0);
+						}
+					}
+					wgmma_commit();
+					wgmma_wait<0>();
+					reg_fence(acc);
+					if (stamp) MLPF_STAMP(s, g - 1, 2);
+					__syncwarp();
+					if (lane == 0) mbar_arrive_plain(bar_w_free + 8 * stage);
+					if (l < NH) {
+						const size_t krow = ((size_t)(BWD ? NH - 1 - l : l) * p.batch_size + row0 + r0) * W + h * C::HALF + 2 * ft;
+						__half* keep = p.hidden_out ? p.hidden_out + krow : nullptr;
+						__half* keep_pre = (PRE && !BWD && kp.hidden_pre_out) ? kp.hidden_pre_out + krow : nullptr;
+#pragma unroll
+						for (uint32_t i = 0; i < C::HALF / 8; ++i) {
+#pragma unroll
+							for (uint32_t hi = 0; hi < 2; ++hi) {
+								const uint32_t lo_bits = __float_as_uint(acc[4 * i + 2 * hi]), hi_bits = __float_as_uint(acc[4 * i + 2 * hi + 1]);
+								uint32_t v;
+								if (PRE && BWD) {
+									v = act_bwd_pre_pack(hid_act, lo_bits, hi_bits, fwd[(2 * i + hi) % (BWD ? C::HALF / 4 : 1)]);
+								} else if (PRE) {
+									const uint32_t z = pack_half2(__uint_as_float(lo_bits), __uint_as_float(hi_bits));
+									if (keep_pre) *reinterpret_cast<uint32_t*>(keep_pre + hi * 8 * W + 8 * i) = z;
+									v = act_pre_pack(hid_act, z);
+								} else {
+									v = BWD ? act_bwd_pack(hid_act, lo_bits, hi_bits, fwd[(2 * i + hi) % (BWD ? C::HALF / 4 : 1)]) : act_pack(hid_act, lo_bits, hi_bits);
+								}
+								if (h == 0) a_lo[i / 2][(i & 1u) * 2 + hi] = v;
+								else a[W / 32 + i / 2][(i & 1u) * 2 + hi] = v;
+								if (keep) *reinterpret_cast<uint32_t*>(keep + hi * 8 * W + 8 * i) = v;
+							}
+						}
+					} else {
+#pragma unroll
+						for (uint32_t i = 0; i < C::HALF / 8; ++i) {
+							const uint32_t c = h * C::HALF + 8 * i + 2 * ft;
+							if (c >= last_w) continue;
+#pragma unroll
+							for (uint32_t hi = 0; hi < 2; ++hi) {
+								const size_t rr = row0 + r0 + hi * 8;
+								const __half2 y = __halves2half2(act_fwd_h(out_act, __float2half_rn(acc[4 * i + 2 * hi])), act_fwd_h(out_act, __float2half_rn(acc[4 * i + 2 * hi + 1])));
+								if (p.output_fp16) *reinterpret_cast<__half2*>(p.output_fp16 + rr * last_w + c) = y;
+								if (p.output_fp32) {
+									if (c < p.n_output_dims) p.output_fp32[rr * p.n_output_dims + c] = __low2float(y);
+									if (c + 1 < p.n_output_dims) p.output_fp32[rr * p.n_output_dims + c + 1] = __high2float(y);
+								}
+							}
+						}
+					}
+					if (stamp) MLPF_STAMP(s, g - 1, 3);
+				}
+				if (l < NH) {
+#pragma unroll
+					for (uint32_t kk = 0; kk < W / 32; ++kk) {
+#pragma unroll
+						for (uint32_t q = 0; q < 4; ++q) a[kk][q] = a_lo[kk][q];
+					}
+				}
+			}
+		}
+	}
+
+	pdl_launch_dependents();
+}
+
 // ------------------------------------------------------------------------------------------------------------------ host side
 namespace {
 
@@ -331,10 +564,49 @@ cudaError_t launch_width(const MlpForwardParams& p, uint32_t n_sms, cudaStream_t
 	return generic ? launch_impl<W, true, false>(p, n_sms, stream) : launch_impl<W, false, false>(p, n_sms, stream);
 }
 
+template <bool GENERIC, bool BWD, bool PRE = false>
+cudaError_t launch_impl256(const MlpForwardParams& p, uint32_t n_sms, cudaStream_t stream) {
+	using C = Mlp256;
+	const uint32_t n_layers = p.n_hidden_layers + ((BWD && !p.output_fp16) ? 0 : 1);
+	MlpKernelParams kp{};
+	kp.p = p;
+	kp.n_steps = n_layers;
+	kp.hidden_pre_out = p.hidden_pre_out;
+	kp.resident = 0;
+	kp.n_stages = C::STAGES;
+	// forward: [128 rows][64 K] boxes (half a matrix's rows); backward: [256 rows][64 N] boxes (all of a matrix's rows = its K)
+	const uint32_t box_rows = BWD ? C::W : C::HALF;
+	CUtensorMap m0, mh, mo;
+	const __half* w = p.weights;
+	if (!make_fp16_matrix_map(&m0, w, C::W, p.in_width, box_rows)) return cudaErrorInvalidValue;
+	w += (size_t)C::W * p.in_width;
+	if (p.n_hidden_layers > 1) {
+		if (!make_fp16_matrix_map(&mh, w, (p.n_hidden_layers - 1) * C::W, C::W, box_rows)) return cudaErrorInvalidValue;
+	} else {
+		mh = m0;  // never used
+	}
+	w += (size_t)(p.n_hidden_layers - 1) * C::W * C::W;
+	if (!make_fp16_matrix_map(&mo, w, p.out_width, C::W, box_rows)) return cudaErrorInvalidValue;
+	auto kernel = mlp_forward256_kernel<GENERIC, BWD, PRE>;
+	const size_t smem = (size_t)C::STAGES * C::STAGE_BYTES + 8 * 2 * MLPF_MAX_STAGES;
+	cudaError_t err = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+	if (err != cudaSuccess) return err;
+	const uint32_t n_groups = (p.batch_size / UNIT_M + C::WGS - 1) / C::WGS;
+	return launch_pdl(kernel, n_groups < n_sms ? n_groups : n_sms, C::THREADS, smem, stream, kp, m0, mh, mo);
+}
+
+cudaError_t launch_width256(const MlpForwardParams& p, uint32_t n_sms, cudaStream_t stream) {
+	if (activation_needs_preact(p.activation)) return p.backward ? launch_impl256<true, true, true>(p, n_sms, stream) : launch_impl256<true, false, true>(p, n_sms, stream);
+	if (p.backward) return p.activation != ACT_RELU ? launch_impl256<true, true>(p, n_sms, stream) : launch_impl256<false, true>(p, n_sms, stream);
+	const bool generic = p.activation != ACT_RELU || p.output_activation != ACT_NONE;
+	return generic ? launch_impl256<true, false>(p, n_sms, stream) : launch_impl256<false, false>(p, n_sms, stream);
+}
+
 }  // namespace
 
 uint32_t mlp_forward_resident_layers(uint32_t width) {
 	switch (width) {
+		case 256: return 0;  // a 256 x 256 matrix is 128 KB: every matrix streams through the ring of half-matrix stages
 		case 128: return max_stages<128>();
 		case 64: return max_stages<64>();
 		case 32: return max_stages<32>();
@@ -347,11 +619,11 @@ bool mlp_forward_supported(const MlpForwardParams& p, const char** why) {
 		if (why) *why = msg;
 		return false;
 	};
-	if (!(p.width == 16 || p.width == 32 || p.width == 64 || p.width == 128)) return fail("FullyFusedMLP only supports 16, 32, 64, and 128 neurons");
+	if (!(p.width == 16 || p.width == 32 || p.width == 64 || p.width == 128 || p.width == 256)) return fail("FullyFusedMLP only supports 16, 32, 64, and 128 neurons");
 	if (p.n_hidden_layers < 1) return fail("FullyFusedMLP requires at least 1 hidden layer (3 layers in total).");
 	if (p.n_hidden_layers + 1 > 64) return fail("tcnn_b200: the stand-alone MLP kernel covers up to 63 hidden layers");
 	const uint32_t max_in = 64 * ((p.width + 63) / 64);
-	if (p.in_width == 0 || p.in_width % 16 != 0 || p.in_width > max_in) return fail("tcnn_b200: network input width must be a multiple of 16 and at most 64 (128 for 128 neurons)");
+	if (p.in_width == 0 || p.in_width % 16 != 0 || p.in_width > max_in) return fail("tcnn_b200: network input width must be a multiple of 16 and at most 64 (128 / 256 for 128 / 256 neurons)");
 	if (p.out_width == 0 || p.out_width % 16 != 0 || p.out_width > p.width) return fail("tcnn_b200: padded network output width must be a multiple of 16 and at most n_neurons");
 	if (p.batch_size == 0 || p.batch_size % TILE_M != 0) return fail("batch size must be a non-zero multiple of 256");
 	if ((p.input_fp16 != nullptr) == (p.input_fp32 != nullptr)) return fail("tcnn_b200: exactly one network input must be given");
@@ -372,6 +644,7 @@ bool mlp_forward_supported(const MlpForwardParams& p, const char** why) {
 cudaError_t launch_mlp_forward(const MlpForwardParams& p, uint32_t n_sms, cudaStream_t stream) {
 	if (!mlp_forward_supported(p, nullptr)) return cudaErrorInvalidValue;
 	switch (p.width) {
+		case 256: return launch_width256(p, n_sms, stream);
 		case 128: return launch_width<128>(p, n_sms, stream);
 		case 64: return launch_width<64>(p, n_sms, stream);
 		case 32: return launch_width<32>(p, n_sms, stream);

@@ -8,7 +8,7 @@ namespace tcnnb {
 struct MlpChainParams {
 	// network (fully_fused_mlp.cu:635-672): W_0 [width][in_width], (n_hidden_layers - 1) x [width][width], W_out [out_width][width],
 	// row-major fp16, contiguous in this order
-	uint32_t width;              // 16 / 32 / 64 / 128
+	uint32_t width;              // 16 / 32 / 64 / 128 / 256
 	uint32_t in_width;           // multiple of 16, <= max(width, 64) ... see mlp_forward_supported()
 	uint32_t out_width;          // PADDED output width: multiple of 16, <= width rounded up to 64
 	uint32_t n_hidden_layers;    // >= 1

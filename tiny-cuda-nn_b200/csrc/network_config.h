@@ -37,9 +37,11 @@ inline MlpConfig parse_network(const json::Value& net, uint32_t in_width, uint32
 	c.activation = parse_activation(net.value("activation", "ReLU"));
 	c.output_activation = parse_activation(net.value("output_activation", "None"));
 	// Both otypes run on the same wgmma kernels (there is no separate non-fused network in this library), so both take the fused
-	// kernel's widths; the reference's CutlassMLP accepts any multiple of 8.
-	if (!(c.width == 16 || c.width == 32 || c.width == 64 || c.width == 128)) {
-		throw std::runtime_error("FullyFusedMLP only supports 16, 32, 64, and 128 neurons, but got " + std::to_string(c.width) + ". Use CutlassMLP instead if this is a requirement.");
+	// kernel's widths, and CutlassMLP also 256 (the width of SIREN and neural-SDF networks); the reference's CutlassMLP accepts any
+	// multiple of 8.
+	if (!(c.width == 16 || c.width == 32 || c.width == 64 || c.width == 128 || (cutlass && c.width == 256))) {
+		const std::string msg = "FullyFusedMLP only supports 16, 32, 64, and 128 neurons, but got " + std::to_string(c.width) + ". Use CutlassMLP instead if this is a requirement.";
+		throw std::runtime_error(cutlass ? msg + " (tcnn_b200's CutlassMLP runs these widths and 256.)" : msg);
 	}
 	if (c.n_hidden_layers < 1) throw std::runtime_error("FullyFusedMLP requires at least 1 hidden layer (3 layers in total).");
 	// Sine and SiLU need stored pre-activations: FullyFusedMLP rejects them (fully_fused_mlp.cu:689-699); CutlassMLP keeps them
