@@ -263,28 +263,6 @@ __global__ void ema_step_kernel(uint32_t n, float decay, float debias_old, float
 	weights_ema[i] = __float2half_rn(filtered);
 }
 
-// Identity encoding on its own (encodings/identity.h:46-67,69-91): rows [n][width] fp16, feature j < n_dims = x_j * scale + offset,
-// padding features 1; and its backward, dL/dx_j = dL/d(feature j) * scale (fp32 rows [n][n_dims]).
-__global__ void identity_encode_kernel(uint64_t n_total, uint32_t n_dims, uint32_t width, float scale, float offset, const float* __restrict__ x, __half* __restrict__ out) {
-	pdl_wait();
-	pdl_launch_dependents();
-	const uint64_t i = threadIdx.x + (uint64_t)blockIdx.x * blockDim.x;
-	if (i >= n_total) return;
-	const uint64_t sample = i / width;
-	const uint32_t j = (uint32_t)(i % width);
-	out[i] = j < n_dims ? __float2half_rn(fmaf(x[sample * n_dims + j], scale, offset)) : __float2half_rn(1.0f);
-}
-
-__global__ void identity_backward_kernel(uint64_t n_total, uint32_t n_dims, uint32_t width, float scale, const __half* __restrict__ dL_dy, float* __restrict__ dL_dx) {
-	pdl_wait();
-	pdl_launch_dependents();
-	const uint64_t i = threadIdx.x + (uint64_t)blockIdx.x * blockDim.x;
-	if (i >= n_total) return;
-	const uint64_t sample = i / n_dims;
-	const uint32_t j = (uint32_t)(i % n_dims);
-	dL_dx[i] = __half2float(dL_dy[sample * width + j]) * scale;
-}
-
 // ------------------------------------------------------------------------------------------------------------------
 // Data parallelism over peer memory. See misc_kernels.h for the protocol.
 // ------------------------------------------------------------------------------------------------------------------
@@ -441,18 +419,6 @@ cudaError_t launch_activation_backward_output(cudaStream_t stream, uint32_t acti
 cudaError_t launch_ema_step(cudaStream_t stream, uint32_t n, float decay, float debias_old, float debias_new, const __half* weights, __half* weights_ema, float* tmp) {
 	if (n == 0) return cudaSuccess;
 	return launch_pdl(ema_step_kernel, blocks_for(n, 256), 256, 0, stream, n, decay, debias_old, debias_new, weights, weights_ema, tmp);
-}
-
-cudaError_t launch_identity_encode(cudaStream_t stream, uint32_t n, uint32_t n_dims, uint32_t width, float scale, float offset, const float* x, __half* out) {
-	const uint64_t total = (uint64_t)n * width;
-	if (total == 0) return cudaSuccess;
-	return launch_pdl(identity_encode_kernel, (uint32_t)((total + 255) / 256), 256, 0, stream, total, n_dims, width, scale, offset, x, out);
-}
-
-cudaError_t launch_identity_backward(cudaStream_t stream, uint32_t n, uint32_t n_dims, uint32_t width, float scale, const __half* dL_dy, float* dL_dx) {
-	const uint64_t total = (uint64_t)n * n_dims;
-	if (total == 0) return cudaSuccess;
-	return launch_pdl(identity_backward_kernel, (uint32_t)((total + 255) / 256), 256, 0, stream, total, n_dims, width, scale, dL_dy, dL_dx);
 }
 
 cudaError_t launch_dp_barrier(cudaStream_t stream, const DpPeers& peers, uint32_t epoch) {

@@ -41,9 +41,6 @@ cudaError_t launch_activation_backward_output(cudaStream_t stream, uint32_t acti
 
 // Ema wrapper (optimizers/ema.h:46-75): weights_ema = (weights_ema * decay * debias_old + weights * (1 - decay)) * debias_new; tmp optional (fp32 average)
 cudaError_t launch_ema_step(cudaStream_t stream, uint32_t n, float decay, float debias_old, float debias_new, const __half* weights, __half* weights_ema, float* tmp);
-// Identity encoding (encodings/identity.h:46-91) as stand-alone kernels: rows [n][width] fp16 with ones as padding; dL/dx in fp32.
-cudaError_t launch_identity_encode(cudaStream_t stream, uint32_t n, uint32_t n_dims, uint32_t width, float scale, float offset, const float* x, __half* out);
-cudaError_t launch_identity_backward(cudaStream_t stream, uint32_t n, uint32_t n_dims, uint32_t width, float scale, const __half* dL_dy, float* dL_dx);
 
 // ---- data parallelism over peer memory (NVLink / NVSwitch): one-pass "reduce + Adam + publish" on this rank's slice ----------------
 // Every rank holds [fp16 params | fp16 gradients | flags] at the SAME offsets of a symmetric allocation that all peers have

@@ -156,7 +156,8 @@ struct Model {
 	bool general = false;
 	bool force_general = false;  // tcnnb_debug_set("general", 1): run the general path although the fused kernel covers the configuration
 	bool use_general() const { return general || force_general; }
-	DeviceBuffer<__half> g_enc, g_hidden, g_out, g_dy, g_grad_hidden, g_denc, g_dy_act;
+	DeviceBuffer<__half> g_enc, g_out, g_dy, g_denc;
+	MlpScratch g_mlp;
 
 	// spatial binning scratch (binning.cu): sorted copies of the batch + permutation
 	bool binning = true;  // tcnnb_debug_set("binning", 0) (tests: binned and unbinned steps must touch the same entries)
@@ -236,19 +237,9 @@ static void init_params(Model& m, HostPcg32& rng, float* dst, float scale) {
 	init_plan_params(m.plan, rng, dst + m.mlp.n_params, scale);  // nested encodings draw one after the other from the same stream
 }
 
-// Whether the stand-alone network kernels cover this network (they have their own limits, e.g. dL/d(encoded) wider than the layers):
-// nullptr, else the reason they do not.
-static const char* general_path_unsupported(const Model& m) {
-	MlpBackwardArgs probe{};
-	probe.width = m.mlp.width;
-	probe.in_width = m.mlp.in_width;
-	probe.out_width = m.mlp.padded_out_width;
-	probe.n_hidden_layers = m.mlp.n_hidden_layers;
-	probe.batch_size = 256;
-	probe.dL_dinput = m.plan.n_params == 0 ? nullptr : (__half*)16;  // the encoding's backward pass needs dL/d(encoded)
-	const char* why_not = nullptr;
-	return mlp_backward_supported(probe, &why_not) ? nullptr : why_not;
-}
+// Whether the stand-alone network kernels cover this network: nullptr, else the reason they do not. The encoding's backward pass
+// needs dL/d(encoded) when it has parameters.
+static const char* general_path_unsupported(const Model& m) { return mlp_unsupported(m.mlp, m.plan.n_params != 0); }
 
 // Whether the fused kernel (fused_ws.cu) covers this configuration: nullptr, else the first of its limits that it does not meet.
 static const char* fused_kernel_unsupported(const EncodingPlan& plan, const MlpConfig& mlp, uint32_t n_in) {
@@ -517,31 +508,11 @@ static void general_forward(Model& m, cudaStream_t stream, uint32_t batch, const
 	const MlpConfig& mlp = m.mlp;
 	grow(m.g_enc, (size_t)batch * mlp.in_width);
 	plan_forward(m.plan, stream, batch, x, params + mlp.n_params, m.g_enc.ptr, mlp.in_width, 1.0f);
-	MlpForwardParams p{};
-	p.width = mlp.width;
-	p.in_width = mlp.in_width;
-	p.out_width = mlp.padded_out_width;
-	p.n_hidden_layers = mlp.n_hidden_layers;
-	p.activation = mlp.activation;
-	p.output_activation = mlp.output_activation;
-	p.weights = params;
-	p.batch_size = batch;
+	MlpForwardParams p = mlp_forward_params(mlp, params, batch, keep_hidden ? m.g_mlp.hidden_rows(mlp, batch) : nullptr);
 	p.input_fp16 = m.g_enc.ptr;
-	p.n_output_dims = m.n_out;
 	p.output_fp16 = out_fp16;
 	p.output_fp32 = out_fp32;
-	if (keep_hidden) {
-		// Sine / SiLU: the pre-activations follow the post-activations in the same buffer
-		const size_t n_hidden = (size_t)mlp.n_hidden_layers * batch * mlp.width;
-		const bool pre = activation_needs_preact(mlp.activation);
-		grow(m.g_hidden, pre ? 2 * n_hidden : n_hidden);
-		p.hidden_out = m.g_hidden.ptr;
-		p.hidden_pre_out = pre ? m.g_hidden.ptr + n_hidden : nullptr;
-	}
-	const char* why = nullptr;
-	if (!mlp_forward_supported(p, &why)) throw std::runtime_error(why);
-	TCNNB_CUDA_CHECK(launch_mlp_forward(p, (uint32_t)m.n_sms, stream));
-	++g_kernel_launches;
+	run_mlp_forward(p, m.n_sms, stream);
 	m.last_stream = stream;
 }
 
@@ -562,50 +533,21 @@ static void general_backward_pass(Model& m, cudaStream_t stream, uint32_t batch,
 	grow(m.g_out, (size_t)batch * mlp.padded_out_width);
 	__half* const out_rows = (m.taps.output && mlp.padded_out_width == 16) ? (__half*)m.taps.output : m.g_out.ptr;  // (the test tap is 16 columns wide)
 	general_forward(m, stream, batch, x, params, out_rows, nullptr, true);
-	const __half* out = out_rows;
 
-	MlpBackwardArgs a{};
-	a.width = mlp.width;
-	a.in_width = mlp.in_width;
-	a.out_width = mlp.padded_out_width;
-	a.n_hidden_layers = mlp.n_hidden_layers;
-	a.activation = mlp.activation;
-	a.weights = params;
-	a.batch_size = batch;
-	a.input = m.g_enc.ptr;
-	a.hidden = m.g_hidden.ptr;
-	if (activation_needs_preact(mlp.activation)) a.hidden_pre = m.g_hidden.ptr + (size_t)mlp.n_hidden_layers * batch * mlp.width;
-	a.output = out;
-	if (ext_dL_doutput) {  // Module::backward: the caller's dL/d(output) still has to pass the output activation (fully_fused_mlp.cu:755-762)
-		a.output_activation = mlp.output_activation;
-		a.dL_doutput = ext_dL_doutput;
-		if (mlp.output_activation != ACT_NONE) {
-			grow(m.g_dy_act, (size_t)batch * mlp.padded_out_width);
-			a.grad_output = m.g_dy_act.ptr;
-		}
-	} else {  // Trainer: loss gradient x loss_scale, through the output activation, in one kernel
+	// Module::backward: the caller's dL/d(output) still has to pass the output activation (fully_fused_mlp.cu:755-762). Trainer: the
+	// loss kernel writes loss gradient x loss_scale, through the output activation, in one kernel.
+	const __half* dL_doutput = ext_dL_doutput;
+	if (!ext_dL_doutput) {
 		grow(m.g_dy, (size_t)batch * mlp.padded_out_width);
-		TCNNB_CUDA_CHECK(launch_loss(stream, m.loss_type, mlp.output_activation, batch, m.n_out, mlp.padded_out_width, m.loss_scale, loss_batch * m.n_out, out, y, m.g_dy.ptr,
+		TCNNB_CUDA_CHECK(launch_loss(stream, m.loss_type, mlp.output_activation, batch, m.n_out, mlp.padded_out_width, m.loss_scale, loss_batch * m.n_out, out_rows, y, m.g_dy.ptr,
 		                             m.taps.loss_values, m.scalars.ptr));
 		++g_kernel_launches;
-		a.output_activation = ACT_NONE;
-		a.dL_doutput = m.g_dy.ptr;
+		dL_doutput = m.g_dy.ptr;
 	}
 	const bool need_denc = grid_params || dL_dinput;
-	if (need_denc) {
-		grow(m.g_denc, (size_t)batch * mlp.in_width);
-		a.dL_dinput = m.g_denc.ptr;
-	}
-	if (want_param_grads) {
-		grow(m.g_grad_hidden, (size_t)mlp.n_hidden_layers * batch * mlp.width);
-		a.grad_hidden = m.g_grad_hidden.ptr;
-		a.dw_accum = m.dw_accum.ptr;
-	}
-	const char* why = nullptr;
-	if (!mlp_backward_supported(a, &why)) throw std::runtime_error(why);
-	uint32_t launches = 0;
-	TCNNB_CUDA_CHECK(launch_mlp_backward(a, (uint32_t)m.n_sms, stream, &launches));
-	g_kernel_launches += launches;
+	if (need_denc) grow(m.g_denc, (size_t)batch * mlp.in_width);
+	run_mlp_backward(mlp, m.g_mlp, m.n_sms, stream, batch, params, m.g_enc.ptr, m.g_mlp.hidden.ptr, out_rows, dL_doutput, ext_dL_doutput != nullptr,
+	                 need_denc ? m.g_denc.ptr : nullptr, want_param_grads ? m.dw_accum.ptr : nullptr);
 	if (want_param_grads) m.mlp_grads_in_accum = true;
 	if (grid_params) plan_param_gradients(m.plan, stream, batch, x, m.g_denc.ptr, mlp.in_width, grads + mlp.n_params, 1.0f);
 	if (dL_dinput) plan_input_gradient(m.plan, stream, batch, x, params + mlp.n_params, m.g_denc.ptr, mlp.in_width, dL_dinput, 1.0f);

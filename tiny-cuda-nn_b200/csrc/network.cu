@@ -1,4 +1,5 @@
-// network.cu -- the stand-alone network tier of the C ABI (include/tcnn_b200.h, tcnnb_network_*).
+// network.cu -- the stand-alone network tier of the C ABI (include/tcnn_b200.h, tcnnb_network_*), and the runner of the stand-alone
+// network kernels that this tier and the general path of model.cu share (network_config.h).
 //
 // Mirrors, for FullyFusedMLP on its own,
 //   src/network.cu:51-141         create_network<T>(json): "otype", "n_neurons", "n_hidden_layers", "activation", "output_activation"
@@ -12,6 +13,7 @@
 // Parameters are CALLER-owned fp16 device arrays, as in the module tier. No fallback: an unsupported shape is an error.
 #include "../../include/tcnn_b200.h"
 
+#include "encoding_plan.h"
 #include "host_common.h"
 #include "json_mini.h"
 #include "misc_kernels.h"
@@ -22,14 +24,97 @@
 
 namespace tcnnb {
 
+// ---- the runner (network_config.h) --------------------------------------------------------------------------------------------
+const char* mlp_unsupported(const MlpConfig& c, bool input_gradient) {
+	MlpBackwardArgs probe{};
+	probe.width = c.width;
+	probe.in_width = c.in_width;
+	probe.out_width = c.padded_out_width;
+	probe.n_hidden_layers = c.n_hidden_layers;
+	probe.batch_size = 256;
+	probe.dL_dinput = input_gradient ? (__half*)16 : nullptr;
+	const char* why_not = nullptr;
+	return mlp_backward_supported(probe, &why_not) ? nullptr : why_not;
+}
+
+// The pre-activation half of a `hidden` buffer (Sine / SiLU), else null.
+template <typename T>
+static T* hidden_pre_of(const MlpConfig& c, T* hidden, uint32_t batch) {
+	return (hidden && activation_needs_preact(c.activation)) ? hidden + (size_t)c.n_hidden_layers * batch * c.width : nullptr;
+}
+
+MlpForwardParams mlp_forward_params(const MlpConfig& c, const __half* weights, uint32_t batch, __half* hidden) {
+	MlpForwardParams p{};
+	p.width = c.width;
+	p.in_width = c.in_width;
+	p.out_width = c.padded_out_width;
+	p.n_hidden_layers = c.n_hidden_layers;
+	p.activation = c.activation;
+	p.output_activation = c.output_activation;
+	p.weights = weights;
+	p.batch_size = batch;
+	p.n_output_dims = c.out_width;
+	p.hidden_out = hidden;
+	p.hidden_pre_out = hidden_pre_of(c, hidden, batch);
+	return p;
+}
+
+void run_mlp_forward(const MlpForwardParams& p, int n_sms, cudaStream_t stream) {
+	const char* why = nullptr;
+	if (!mlp_forward_supported(p, &why)) throw std::runtime_error(why);
+	TCNNB_CUDA_CHECK(launch_mlp_forward(p, (uint32_t)n_sms, stream));
+	++g_kernel_launches;
+}
+
+__half* MlpScratch::hidden_rows(const MlpConfig& c, uint32_t batch) {
+	grow(hidden, (size_t)n_forward_activations(c) * batch * c.width);
+	return hidden.ptr;
+}
+
+void run_mlp_backward(const MlpConfig& c, MlpScratch& s, int n_sms, cudaStream_t stream, uint32_t batch, const __half* weights, const __half* input, const __half* hidden,
+                      const __half* output, const __half* dL_doutput, bool apply_output_activation, __half* dL_dinput, float* dw_accum) {
+	MlpBackwardArgs a{};
+	a.width = c.width;
+	a.in_width = c.in_width;
+	a.out_width = c.padded_out_width;
+	a.n_hidden_layers = c.n_hidden_layers;
+	a.activation = c.activation;
+	a.output_activation = apply_output_activation ? c.output_activation : (uint32_t)ACT_NONE;
+	a.weights = weights;
+	a.batch_size = batch;
+	a.input = input;
+	a.hidden = hidden;
+	a.hidden_pre = hidden_pre_of(c, hidden, batch);
+	a.output = output;
+	a.dL_doutput = dL_doutput;
+	a.dL_dinput = dL_dinput;
+	if (dw_accum) {
+		grow(s.grad_hidden, (size_t)c.n_hidden_layers * batch * c.width);
+		a.grad_hidden = s.grad_hidden.ptr;
+		a.dw_accum = dw_accum;
+	}
+	if (a.output_activation != ACT_NONE) {
+		grow(s.grad_output, (size_t)batch * c.padded_out_width);
+		a.grad_output = s.grad_output.ptr;
+	}
+	const char* why = nullptr;
+	if (!mlp_backward_supported(a, &why)) throw std::runtime_error(why);
+	uint32_t launches = 0;
+	TCNNB_CUDA_CHECK(launch_mlp_backward(a, (uint32_t)n_sms, stream, &launches));
+	g_kernel_launches += launches;
+}
+
+// ---- the network tier ---------------------------------------------------------------------------------------------------------
 struct Network {
 	uint32_t n_input_dims = 0;   // cfg.in_width rounds it up to 16 (the Identity encoding pads with ones)
 	MlpConfig cfg;
+	EncodingPlan identity;       // the Identity encoding in front of the network (module_backward), identity.width == cfg.in_width
 	int n_sms = 132;
 	long long* dbg_clock = nullptr;  // profiling only (tcnnb_network_debug_clocks)
-	// scratch of the backward pass (grown on demand, reused): g_l rows, dL/d(output) through the output activation, fp32 weight-gradient
-	// sums, and -- module tier, fp32 inputs -- the Identity-encoded input rows, the recomputed activations and dL/d(encoded input)
-	DeviceBuffer<__half> grad_hidden, grad_output, enc_input, hidden, output, grad_input;
+	MlpScratch scratch;
+	// module_backward (fp32 inputs): the Identity-encoded input rows, the recomputed output and dL/d(encoded input); fp32 weight-
+	// gradient sums of the backward pass
+	DeviceBuffer<__half> enc_input, output, grad_input;
 	DeviceBuffer<float> dw_accum;
 };
 
@@ -38,51 +123,22 @@ static void build_network(Network& n, uint32_t n_in, uint32_t n_out, const json:
 	n.cfg = parse_network(net, next_multiple(n_in, 16u), n_out);
 	if (n_in == 0 || n_out == 0) throw std::runtime_error("network: n_input_dims and n_output_dims must be positive.");
 	n.n_input_dims = n_in;
-	MlpForwardParams probe{};
-	probe.width = n.cfg.width;
-	probe.in_width = n.cfg.in_width;
-	probe.out_width = n.cfg.padded_out_width;
-	probe.n_hidden_layers = n.cfg.n_hidden_layers;
-	probe.batch_size = 256;
-	probe.input_fp16 = (const __half*)16;
-	const char* why = nullptr;
-	if (!mlp_forward_supported(probe, &why)) throw std::runtime_error(why);
+	build_encoding_plan(n.identity, n_in, json::parse("{\"otype\": \"Identity\"}"), 16);
+	if (const char* why = mlp_unsupported(n.cfg, false)) throw std::runtime_error(why);
 }
 
-// Hidden rows per hidden layer the forward pass keeps for the backward pass (CutlassMLP::num_forward_activations()): the post-
-// activations, and for Sine / SiLU the pre-activations after them.
-static uint32_t n_forward_activations(const MlpConfig& c) { return activation_needs_preact(c.activation) ? 2 * c.n_hidden_layers : c.n_hidden_layers; }
-
-// The pre-activation half of a `hidden` buffer [2][n_hidden_layers][batch][width] (Sine / SiLU), else null.
-template <typename T>
-static T* hidden_pre_of(const MlpConfig& c, T* hidden, uint32_t batch) {
-	return (hidden && activation_needs_preact(c.activation)) ? hidden + (size_t)c.n_hidden_layers * batch * c.width : nullptr;
-}
-
-static MlpForwardParams make_params(const Network& n, uint32_t batch, const void* params) {
+static void check_args(uint32_t batch, const void* params) {
 	check_batch(batch);
 	if (!params) throw std::runtime_error("network: params is null.");
 	if ((uintptr_t)params % 16 != 0) throw std::runtime_error("network: params must be 16-byte aligned.");
-	MlpForwardParams p{};
-	p.width = n.cfg.width;
-	p.in_width = n.cfg.in_width;
-	p.out_width = n.cfg.padded_out_width;
-	p.n_hidden_layers = n.cfg.n_hidden_layers;
-	p.activation = n.cfg.activation;
-	p.output_activation = n.cfg.output_activation;
-	p.weights = (const __half*)params;
-	p.batch_size = batch;
-	p.n_input_dims = n.n_input_dims;
-	p.n_output_dims = n.cfg.out_width;
-	p.dbg_clock = n.dbg_clock;
-	return p;
 }
 
-static void launch(const Network& n, const MlpForwardParams& p, cudaStream_t stream) {
-	const char* why = nullptr;
-	if (!mlp_forward_supported(p, &why)) throw std::runtime_error(why);
-	TCNNB_CUDA_CHECK(launch_mlp_forward(p, (uint32_t)n.n_sms, stream));
-	++g_kernel_launches;
+static MlpForwardParams make_params(const Network& n, uint32_t batch, const void* params, __half* hidden = nullptr) {
+	check_args(batch, params);
+	MlpForwardParams p = mlp_forward_params(n.cfg, (const __half*)params, batch, hidden);
+	p.n_input_dims = n.n_input_dims;
+	p.dbg_clock = n.dbg_clock;
+	return p;
 }
 
 // Network<T>::backward (fully_fused_mlp.cu:733-866): dL/d(input) (fp16 rows, optional) and dL/d(params) (fp16, OVERWRITTEN, optional)
@@ -90,47 +146,18 @@ static void launch(const Network& n, const MlpForwardParams& p, cudaStream_t str
 static void network_backward(Network& n, cudaStream_t stream, uint32_t batch, const __half* input, const __half* output, const __half* hidden, const __half* dL_doutput,
                              const void* params, __half* dL_dinput, __half* dL_dparams) {
 	if (!dL_dinput && !dL_dparams) return;
-	MlpForwardParams probe = make_params(n, batch, params);  // validates batch / params
-	(void)probe;
+	check_args(batch, params);
 	if (!input || !hidden || !dL_doutput) throw std::runtime_error("network: backward needs the forward pass's input and hidden activations and dL_doutput.");
 	if (n.cfg.output_activation != ACT_NONE && !output) throw std::runtime_error("network: backward through an output activation needs the forward pass's output.");
-	MlpBackwardArgs a{};
-	a.width = n.cfg.width;
-	a.in_width = n.cfg.in_width;
-	a.out_width = n.cfg.padded_out_width;
-	a.n_hidden_layers = n.cfg.n_hidden_layers;
-	a.activation = n.cfg.activation;
-	a.output_activation = n.cfg.output_activation;
-	a.weights = (const __half*)params;
-	a.batch_size = batch;
-	a.input = input;
-	a.hidden = hidden;
-	a.hidden_pre = hidden_pre_of(n.cfg, hidden, batch);
-	a.output = output;
-	a.dL_doutput = dL_doutput;
-	a.dL_dinput = dL_dinput;
-	if (dL_dparams) {
-		grow(n.grad_hidden, (size_t)n.cfg.n_hidden_layers * batch * n.cfg.width);
-		a.grad_hidden = n.grad_hidden.ptr;
-		if (n.dw_accum.n != n.cfg.n_params) {
-			n.dw_accum.resize(n.cfg.n_params);
-			n.dw_accum.zero(stream);  // launch_mlp_grad_finalize re-zeroes it after every use
-		}
-		a.dw_accum = n.dw_accum.ptr;
+	if (dL_dparams && n.dw_accum.n != n.cfg.n_params) {
+		n.dw_accum.resize(n.cfg.n_params);
+		n.dw_accum.zero(stream);  // launch_mlp_grad_finalize re-zeroes it after every use
 	}
-	if (n.cfg.output_activation != ACT_NONE) {
-		grow(n.grad_output, (size_t)batch * n.cfg.padded_out_width);
-		a.grad_output = n.grad_output.ptr;
-	}
-	const char* why = nullptr;
-	if (!mlp_backward_supported(a, &why)) throw std::runtime_error(why);
-	uint32_t launches = 0;
-	TCNNB_CUDA_CHECK(launch_mlp_backward(a, (uint32_t)n.n_sms, stream, &launches));
+	run_mlp_backward(n.cfg, n.scratch, n.n_sms, stream, batch, (const __half*)params, input, hidden, output, dL_doutput, true, dL_dinput, dL_dparams ? n.dw_accum.ptr : nullptr);
 	if (dL_dparams) {
 		TCNNB_CUDA_CHECK(launch_mlp_grad_finalize(stream, (uint32_t)n.cfg.n_params, n.dw_accum.ptr, dL_dparams));
-		++launches;
+		++g_kernel_launches;
 	}
-	g_kernel_launches += launches;
 }
 
 }  // namespace tcnnb
@@ -186,7 +213,7 @@ int tcnnb_network_inference_mixed_precision(tcnnb_network* n, tcnnb_stream strea
 	MlpForwardParams p = make_params(net, n_elements, params_dev);
 	p.input_fp16 = (const __half*)input_dev;
 	p.output_fp16 = (__half*)output_dev;
-	launch(net, p, (cudaStream_t)stream);
+	run_mlp_forward(p, net.n_sms, (cudaStream_t)stream);
 	TCNNB_API_END
 }
 
@@ -196,12 +223,10 @@ int tcnnb_network_forward(tcnnb_network* n, tcnnb_stream stream, uint32_t n_elem
 	if (net.n_input_dims != net.cfg.in_width) throw std::runtime_error("network: fp16 inputs need n_input_dims to be a multiple of 16.");
 	if (!input_dev) throw std::runtime_error("network: input is null.");
 	if (((uintptr_t)input_dev | (uintptr_t)output_dev | (uintptr_t)hidden_dev) % 16 != 0) throw std::runtime_error("network: input / output / hidden must be 16-byte aligned.");
-	MlpForwardParams p = make_params(net, n_elements, params_dev);
+	MlpForwardParams p = make_params(net, n_elements, params_dev, (__half*)hidden_dev);
 	p.input_fp16 = (const __half*)input_dev;
 	p.output_fp16 = (__half*)output_dev;
-	p.hidden_out = (__half*)hidden_dev;
-	p.hidden_pre_out = hidden_pre_of(net.cfg, (__half*)hidden_dev, n_elements);
-	launch(net, p, (cudaStream_t)stream);
+	run_mlp_forward(p, net.n_sms, (cudaStream_t)stream);
 	TCNNB_API_END
 }
 
@@ -228,27 +253,21 @@ int tcnnb_network_module_backward(tcnnb_network* n, tcnnb_stream stream_, uint32
 	if (!dL_dinput_dev && !dL_dparams_dev) return 0;
 	if (!input_dev || !dL_doutput_dev) throw std::runtime_error("network: input / dL_doutput is null.");
 	if (((uintptr_t)dL_doutput_dev | (uintptr_t)dL_dparams_dev) % 16 != 0) throw std::runtime_error("network: dL_doutput / dL_dparams must be 16-byte aligned.");
-	MlpForwardParams p = make_params(net, n_elements, params_dev);
+	check_args(n_elements, params_dev);  // before any scratch is sized by n_elements
+	MlpForwardParams p = make_params(net, n_elements, params_dev, net.scratch.hidden_rows(net.cfg, n_elements));
 	grow(net.enc_input, (size_t)n_elements * net.cfg.in_width);
-	grow(net.hidden, (size_t)n_forward_activations(net.cfg) * n_elements * net.cfg.width);
 	grow(net.output, (size_t)n_elements * net.cfg.padded_out_width);
-	TCNNB_CUDA_CHECK(launch_identity_encode(stream, n_elements, net.n_input_dims, net.cfg.in_width, 1.0f, 0.0f, input_dev, net.enc_input.ptr));
-	++g_kernel_launches;
+	plan_forward(net.identity, stream, n_elements, input_dev, nullptr, net.enc_input.ptr, net.cfg.in_width, 1.0f);
 	p.input_fp16 = net.enc_input.ptr;
 	p.output_fp16 = net.output.ptr;
-	p.hidden_out = net.hidden.ptr;
-	p.hidden_pre_out = hidden_pre_of(net.cfg, net.hidden.ptr, n_elements);
-	launch(net, p, stream);
+	run_mlp_forward(p, net.n_sms, stream);
 	__half* dL_denc = nullptr;
 	if (dL_dinput_dev) {
 		grow(net.grad_input, (size_t)n_elements * net.cfg.in_width);
 		dL_denc = net.grad_input.ptr;
 	}
-	network_backward(net, stream, n_elements, net.enc_input.ptr, net.output.ptr, net.hidden.ptr, (const __half*)dL_doutput_dev, params_dev, dL_denc, (__half*)dL_dparams_dev);
-	if (dL_dinput_dev) {
-		TCNNB_CUDA_CHECK(launch_identity_backward(stream, n_elements, net.n_input_dims, net.cfg.in_width, 1.0f, dL_denc, dL_dinput_dev));
-		++g_kernel_launches;
-	}
+	network_backward(net, stream, n_elements, net.enc_input.ptr, net.output.ptr, p.hidden_out, (const __half*)dL_doutput_dev, params_dev, dL_denc, (__half*)dL_dparams_dev);
+	if (dL_dinput_dev) plan_input_gradient(net.identity, stream, n_elements, input_dev, nullptr, dL_denc, net.cfg.in_width, dL_dinput_dev, 1.0f);
 	TCNNB_API_END
 }
 
@@ -260,7 +279,7 @@ int tcnnb_network_module_inference(tcnnb_network* n, tcnnb_stream stream, uint32
 	MlpForwardParams p = make_params(net, n_elements, params_dev);
 	p.input_fp32 = input_dev;
 	p.output_fp16 = (__half*)output_dev;
-	launch(net, p, (cudaStream_t)stream);
+	run_mlp_forward(p, net.n_sms, (cudaStream_t)stream);
 	TCNNB_API_END
 }
 
@@ -271,7 +290,7 @@ int tcnnb_network_inference(tcnnb_network* n, tcnnb_stream stream, uint32_t n_el
 	MlpForwardParams p = make_params(net, n_elements, params_dev);
 	p.input_fp32 = input_dev;
 	p.output_fp32 = output_dev;
-	launch(net, p, (cudaStream_t)stream);
+	run_mlp_forward(p, net.n_sms, (cudaStream_t)stream);
 	TCNNB_API_END
 }
 

@@ -1,10 +1,12 @@
 // network_config.h -- host-side description of the MLP behind every tier (model.cu: trainer / module tiers; network.cu: the
 // stand-alone network tier): the "network" JSON with the reference's keys, defaults and error texts (src/network.cu:51-141), the
-// parameter layout and the xavier initialisation (fully_fused_mlp.cu:635-672, 868-892).
+// parameter layout and the xavier initialisation (fully_fused_mlp.cu:635-672, 868-892), and the runner of the stand-alone network
+// kernels that the network tier and the general path share.
 #pragma once
 #include "common.cuh"
 #include "host_common.h"
 #include "json_mini.h"
+#include "mlp_fused.h"
 
 #include <cmath>
 #include <string>
@@ -80,5 +82,34 @@ inline void init_mlp_params(const MlpConfig& c, HostPcg32& rng, float* dst, floa
 	}
 	TCNNB_CUDA_CHECK(cudaMemcpy(dst, w.data(), sizeof(float) * w.size(), cudaMemcpyHostToDevice));
 }
+
+// ---- runner of the stand-alone network kernels (mlp_fused.cu / mlp_wgrad.cu), defined in network.cu. The activations a forward pass
+// keeps for the backward pass are `hidden` [n_forward_activations][batch][width]: the post-activations of every hidden layer, and for
+// Sine / SiLU the pre-activations after them (CutlassMLP::num_forward_activations(), cutlass_mlp.cu:162-209).
+inline uint32_t n_forward_activations(const MlpConfig& c) { return activation_needs_preact(c.activation) ? 2 * c.n_hidden_layers : c.n_hidden_layers; }
+
+// Whether the kernels cover this network's shape (they have their own limits, e.g. dL/d(input) wider than the layers): nullptr, else
+// the reason they do not. `input_gradient`: the backward pass has to produce dL/d(input).
+const char* mlp_unsupported(const MlpConfig& c, bool input_gradient);
+
+// Forward-pass arguments for `batch` rows; with `hidden`, the pass keeps its activations there. The caller sets input and output.
+MlpForwardParams mlp_forward_params(const MlpConfig& c, const __half* weights, uint32_t batch, __half* hidden = nullptr);
+// Throws the kernel's reason if it does not cover `p`, else launches it (adds to g_kernel_launches).
+void run_mlp_forward(const MlpForwardParams& p, int n_sms, cudaStream_t stream);
+
+// Scratch of a tier that runs backward passes, grown on demand and reused.
+struct MlpScratch {
+	DeviceBuffer<__half> hidden;       // activations kept by a forward pass (hidden_rows)
+	DeviceBuffer<__half> grad_hidden;  // g_l = dL/d(pre-activation of hidden layer l), for the weight gradients
+	DeviceBuffer<__half> grad_output;  // dL/d(output) through the output activation
+	__half* hidden_rows(const MlpConfig& c, uint32_t batch);
+};
+
+// Network<T>::backward (fully_fused_mlp.cu:733-866) from a forward pass's input, `hidden` and output: dL/d(input) (fp16 rows) into
+// `dL_dinput` and the weight gradients ADDED into the fp32 sums `dw_accum`; either may be null. `apply_output_activation`: dL_doutput
+// has yet to pass the output activation's derivative. Throws the kernels' reason if they do not cover the call, else launches them
+// (adds to g_kernel_launches).
+void run_mlp_backward(const MlpConfig& c, MlpScratch& s, int n_sms, cudaStream_t stream, uint32_t batch, const __half* weights, const __half* input, const __half* hidden,
+                      const __half* output, const __half* dL_doutput, bool apply_output_activation, __half* dL_dinput, float* dw_accum);
 
 }  // namespace tcnnb
