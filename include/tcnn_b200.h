@@ -89,6 +89,21 @@ int tcnnb_set_optimizer_progress(tcnnb_model* m, uint32_t current_step, float ba
  * input_dev [batch][n_in] fp32, target_dev [batch][n_out] fp32, both device pointers.
  * Runs fwd + loss + bwd (+ Adam when run_optimizer != 0). The loss of this step is fetched with tcnnb_loss. */
 int tcnnb_training_step(tcnnb_model* m, tcnnb_stream stream, uint32_t batch_size, const float* input_dev, const float* target_dev, int run_optimizer);
+/* trainer->training_step(stream, input, target, data_pdf, run_optimizer, dL_dinput, use_inference_params, param_gradients_mode,
+ *                        external_dL_dy)  (trainer.h:254-357). Device pointers; every one but input_dev may be null.
+ *   data_pdf_dev        fp32 [batch][n_out], laid out like the targets: every loss divides by the sample's pdf (losses/l2.h etc.; Variance's
+ *                       value is factor / pred - factor / pdf with factor = target^2 / pdf / n_total, variance_is.h:69-76).
+ *   dL_dinput_dev       fp32 [batch][n_in], overwritten with dL/d(input).
+ *   use_inference_params  forward and backward read tcnnb_params_inference (the Ema weights); gradients still go to the trainer.
+ *   param_gradients_mode  0 Ignore (the gradient buffer is left as it is), 1 Overwrite (tcnnb_training_step), 2 Accumulate (adds this
+ *                       step's gradients onto the buffer, also after tcnnb_param_gradients) -- GradientMode, object.h:116-120.
+ *   external_dL_dy_dev  fp16 [batch][padded_output_width], already multiplied by the loss scale (tcnnb_default_loss_scale): replaces
+ *                       the loss (trainer.h:127-131), so target_dev and data_pdf_dev are not read. It still passes through the output
+ *                       activation's transfer. The reference leaves the loss values of such a step unfilled; tcnnb_loss returns 0.
+ * Rejected: handles of tcnnb_module_create, handles with a data-parallel state (tcnnb_dp_init), a null target without
+ * external_dL_dy, batches that are not a multiple of tcnnb_batch_size_granularity(). */
+int tcnnb_training_step_ex(tcnnb_model* m, tcnnb_stream stream, uint32_t batch_size, const float* input_dev, const float* target_dev, const float* data_pdf_dev,
+                           int run_optimizer, float* dL_dinput_dev, int use_inference_params, int param_gradients_mode, const void* external_dL_dy_dev);
 /* Data-parallel variant: this rank's shard of a global batch; the loss is normalised over global_batch_size
  * (loss n_total, relative_l2.h:62) so that gradient sums over ranks equal the single-GPU gradients. */
 int tcnnb_training_step_shard(tcnnb_model* m, tcnnb_stream stream, uint32_t shard_batch_size, uint32_t global_batch_size, const float* input_dev, const float* target_dev, int run_optimizer);

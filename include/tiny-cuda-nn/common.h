@@ -38,6 +38,14 @@ static constexpr MatrixLayout CM = MatrixLayout::ColumnMajor;
 		if (_result != cudaSuccess) throw std::runtime_error{std::string(#x " failed: ") + cudaGetErrorString(_result)};   \
 	} while (0)
 
+/* common_host.h:71-72 */
+#ifndef CHECK_THROW
+#define TCNNB_STR_(x) #x
+#define TCNNB_STR(x) TCNNB_STR_(x)
+#define CHECK_THROW(x) \
+	do { if (!(x)) throw std::runtime_error{__FILE__ ":" TCNNB_STR(__LINE__) " check failed: " #x}; } while (0)
+#endif
+
 #define TCNNB_CHECK_THROW(x)                                                                                              \
 	do {                                                                                                                   \
 		if ((x) != 0) throw std::runtime_error{tcnnb_last_error()};                                                        \

@@ -25,6 +25,7 @@
 #include "common.h"
 #include "gpu_matrix.h"
 #include "gpu_memory.h"
+#include "object.h"
 #include "random.h"
 
 namespace tcnn {
@@ -118,16 +119,47 @@ public:
 		m_model->attach(m_handle);
 	}
 
-	/* trainer.h:254-357 (input / target: n_dims x batch, column-major fp32; data_pdf, dL_dinput, external_dL_dy not supported) */
+	/* trainer.h:254-357. Matrices are n_dims x batch, column-major: input, target, data_pdf and dL_dinput fp32, external_dL_dy
+	 * COMPUTE_T (fp16) padded_output_width x batch and already multiplied by the loss scale. With external_dL_dy the loss is not
+	 * evaluated (target and data_pdf are not read) and loss() returns 0. */
 	std::unique_ptr<Context> training_step(cudaStream_t stream, const GPUMatrixDynamic<T>& input, const GPUMatrixDynamic<float>& target, const GPUMatrixDynamic<float>* data_pdf = nullptr,
-	                                       bool run_optimizer = true) {
-		if (data_pdf) throw std::runtime_error{"training_step: data_pdf is not supported"};
-		if (input.n() != target.n()) throw std::runtime_error{"training_step: input and target batch sizes differ"};
-		if (input.layout() != CM || target.layout() != CM) throw std::runtime_error{"training_step: column-major (sample-contiguous) matrices only"};
-		TCNNB_CHECK_THROW(tcnnb_training_step(m_handle->m, (tcnnb_stream)stream, input.n(), input.data(), target.data(), run_optimizer ? 1 : 0));
+	                                       bool run_optimizer = true, GPUMatrixDynamic<T>* dL_dinput = nullptr, bool use_inference_params = false,
+	                                       GradientMode param_gradients_mode = GradientMode::Overwrite, const GPUMatrixDynamic<COMPUTE_T>* external_dL_dy = nullptr) {
+		if (!data_pdf && !dL_dinput && !use_inference_params && param_gradients_mode == GradientMode::Overwrite && !external_dL_dy) {
+			if (input.n() != target.n()) throw std::runtime_error{"training_step: input and target batch sizes differ"};
+			if (input.layout() != CM || target.layout() != CM) throw std::runtime_error{"training_step: column-major (sample-contiguous) matrices only"};
+			TCNNB_CHECK_THROW(tcnnb_training_step(m_handle->m, (tcnnb_stream)stream, input.n(), input.data(), target.data(), run_optimizer ? 1 : 0));
+			return std::make_unique<Context>();
+		}
+		const uint32_t batch_size = input.n();
+		if (input.layout() != CM) throw std::runtime_error{"training_step: column-major (sample-contiguous) matrices only"};
+		if (external_dL_dy) {  /* trainer.h:127-131 */
+			CHECK_THROW(external_dL_dy->m() == m_model->padded_output_width());
+			CHECK_THROW(external_dL_dy->n() == batch_size);
+			if (external_dL_dy->layout() != CM) throw std::runtime_error{"training_step: column-major (sample-contiguous) matrices only"};
+		} else {  /* trainer.h:133-138, losses/relative_l2.h:93-96 */
+			CHECK_THROW(input.n() == target.n());
+			CHECK_THROW(m_model->output_width() == target.m());
+			const uint32_t dims = target.m();
+			CHECK_THROW(!data_pdf || data_pdf->m() == dims);
+			CHECK_THROW(!data_pdf || data_pdf->n() == batch_size);
+			if (target.layout() != CM || (data_pdf && data_pdf->layout() != CM)) throw std::runtime_error{"training_step: column-major (sample-contiguous) matrices only"};
+		}
+		if (dL_dinput) {
+			CHECK_THROW(dL_dinput->m() == m_model->input_width());
+			CHECK_THROW(dL_dinput->n() == batch_size);
+			if (dL_dinput->layout() != CM) throw std::runtime_error{"training_step: column-major (sample-contiguous) matrices only"};
+		}
+		TCNNB_CHECK_THROW(tcnnb_training_step_ex(m_handle->m, (tcnnb_stream)stream, batch_size, input.data(), external_dL_dy ? nullptr : target.data(),
+		                                         external_dL_dy || !data_pdf ? nullptr : data_pdf->data(), run_optimizer ? 1 : 0, dL_dinput ? dL_dinput->data() : nullptr,
+		                                         use_inference_params ? 1 : 0, (int)param_gradients_mode, external_dL_dy ? external_dL_dy->data() : nullptr));
 		return std::make_unique<Context>();
 	}
-	std::unique_ptr<Context> training_step(const GPUMatrixDynamic<T>& input, const GPUMatrixDynamic<float>& target) { return training_step(nullptr, input, target); }
+	std::unique_ptr<Context> training_step(const GPUMatrixDynamic<T>& input, const GPUMatrixDynamic<float>& target, const GPUMatrixDynamic<float>* data_pdf = nullptr,
+	                                       bool run_optimizer = true, GPUMatrixDynamic<T>* dL_dinput = nullptr, bool use_inference_params = false,
+	                                       GradientMode param_gradients_mode = GradientMode::Overwrite, const GPUMatrixDynamic<COMPUTE_T>* external_dL_dy = nullptr) {
+		return training_step(nullptr, input, target, data_pdf, run_optimizer, dL_dinput, use_inference_params, param_gradients_mode, external_dL_dy);
+	}
 
 	void optimizer_step(cudaStream_t stream, float /*loss_scale*/) { TCNNB_CHECK_THROW(tcnnb_optimizer_step(m_handle->m, (tcnnb_stream)stream)); } /* trainer.h:155-157 */
 

@@ -156,6 +156,19 @@ __device__ __forceinline__ void loss_element(uint32_t loss_type, float pred, flo
 	}
 }
 
+// loss_element with the sample's data_pdf (losses/*.h): value and gradient of the plain loss divided by the pdf -- except Variance's
+// value, which is factor / pred - factor / pdf with factor = target^2 / pdf / n_total (variance_is.h:69-76).
+__device__ __forceinline__ void loss_element_pdf(uint32_t loss_type, float pred, float target, float pdf, float n_total, float luminance, float& value, float& grad) {
+	loss_element(loss_type, pred, target, n_total, luminance, value, grad);
+	grad /= pdf;
+	if (loss_type == LOSS_VARIANCE_IS) {
+		const float factor = target * target / pdf / n_total;
+		value = factor / pred - factor / pdf;
+	} else {
+		value /= pdf;
+	}
+}
+
 // 0.299 r + 0.587 g + 0.114 b of a row of predictions; with 6 or more outputs, channels 3..5 are added to 0..2 first
 // (relative_l2_luminance.h:69-77). `row`: the first 6 predictions of the sample.
 __device__ __forceinline__ float row_luminance(const __half* row, uint32_t dims) {

@@ -50,6 +50,8 @@ struct FusedStepParams {
 	__half* dbg_grad_hidden;       // [n_hidden][batch][64]
 	__half* dbg_denc;              // [batch][64]
 	long long* dbg_clock;          // ablation builds: [cta][role 3][tile 16][slot 16] clock64 stamps of the ws kernel's phases
+	// Last, so that the kernels without it keep their parameter offsets.
+	const float* data_pdf;         // [batch][n_out] fp32, optional: the loss divides by it (Trainer::training_step's data_pdf)
 };
 
 // Shared memory of the fused kernel: encoded / hidden / dy tiles of 128 x 64 fp16 (an encoding of at most 32 features parks its

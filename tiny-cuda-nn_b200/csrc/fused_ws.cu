@@ -74,7 +74,8 @@ __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t n_threads) 
 
 }  // namespace
 
-template <uint32_t D, uint32_t F, bool TRAIN, bool GENERIC_ACT>
+// PDF: the loss divides by p.data_pdf (a flag of its own, so that the kernels without it carry no null check)
+template <uint32_t D, uint32_t F, bool TRAIN, bool GENERIC_ACT, bool PDF>
 __global__ void __launch_bounds__(WS_THREADS, 1) fused_ws_kernel(const FusedStepParams p) {
 	// ReLU hidden / linear output (the reference's default and the benchmark configuration) fold to the packed fast path at compile time
 	const uint32_t hid_act = GENERIC_ACT ? p.activation : (uint32_t)ACT_RELU;
@@ -611,7 +612,8 @@ __global__ void __launch_bounds__(WS_THREADS, 1) fused_ws_kernel(const FusedStep
 								const float pred = __half2float(y16[q]);
 								const float target = q < N_TGT_PREFETCH ? tgt[q] : __ldg(p.targets + (size_t)osample * p.n_out + q);
 								float value, grad;
-								loss_element(p.loss_type, pred, target, n_total, luminance, value, grad);
+								if constexpr (PDF) loss_element_pdf(p.loss_type, pred, target, __ldg(p.data_pdf + (size_t)osample * p.n_out + q), n_total, luminance, value, grad);
+								else loss_element(p.loss_type, pred, target, n_total, luminance, value, grad);
 								gq = p.loss_scale * grad / n_total;
 								loss_acc += value;
 								if (p.loss_values) p.loss_values[(size_t)osample * p.n_out + q] = value;
@@ -699,9 +701,9 @@ size_t fused_ws_smem_bytes(uint32_t n_hidden_layers, uint32_t enc_width, bool tr
 	return fused_ws_base_smem_bytes(n_hidden_layers, enc_width, train) + (train && fused_ws_dw_in_smem(n_hidden_layers, enc_width) ? fused_ws_dw_bytes(n_hidden_layers) : 0);
 }
 
-template <uint32_t D, bool TRAIN, bool GENERIC>
+template <uint32_t D, bool TRAIN, bool GENERIC, bool PDF>
 static cudaError_t launch_ws_impl(const FusedStepParams& p, uint32_t n_ctas, cudaStream_t stream) {
-	auto kernel = fused_ws_kernel<D, 2, TRAIN, GENERIC>;
+	auto kernel = fused_ws_kernel<D, 2, TRAIN, GENERIC, PDF>;
 	const size_t smem = fused_ws_smem_bytes(p.n_hidden_layers, p.grid.padded_width, TRAIN);
 	cudaError_t err = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
 	if (err != cudaSuccess) return err;
@@ -712,15 +714,22 @@ static cudaError_t launch_ws_impl(const FusedStepParams& p, uint32_t n_ctas, cud
 	return launch_pdl(kernel, n_ctas, WS_THREADS, smem, stream, p);
 }
 
-template <uint32_t D, bool TRAIN>
+template <uint32_t D, bool TRAIN, bool PDF>
 static cudaError_t launch_ws_act(const FusedStepParams& p, uint32_t n_ctas, cudaStream_t stream) {
 	const bool generic = p.activation != ACT_RELU || p.output_activation != ACT_NONE;
-	return generic ? launch_ws_impl<D, TRAIN, true>(p, n_ctas, stream) : launch_ws_impl<D, TRAIN, false>(p, n_ctas, stream);
+	return generic ? launch_ws_impl<D, TRAIN, true, PDF>(p, n_ctas, stream) : launch_ws_impl<D, TRAIN, false, PDF>(p, n_ctas, stream);
+}
+
+// the pdf is read by the loss only: inference and steps on a caller's dL/d(output) run the kernels without it
+template <uint32_t D, bool TRAIN>
+static cudaError_t launch_ws_pdf(const FusedStepParams& p, uint32_t n_ctas, cudaStream_t stream) {
+	if (TRAIN && p.data_pdf && !p.ext_dy) return launch_ws_act<D, TRAIN, TRAIN>(p, n_ctas, stream);
+	return launch_ws_act<D, TRAIN, false>(p, n_ctas, stream);
 }
 
 cudaError_t launch_fused_ws(const FusedStepParams& p, uint32_t n_pos_dims, bool train, uint32_t n_ctas, cudaStream_t stream) {
-	if (n_pos_dims == 3) return train ? launch_ws_act<3, true>(p, n_ctas, stream) : launch_ws_act<3, false>(p, n_ctas, stream);
-	if (n_pos_dims == 2) return train ? launch_ws_act<2, true>(p, n_ctas, stream) : launch_ws_act<2, false>(p, n_ctas, stream);
+	if (n_pos_dims == 3) return train ? launch_ws_pdf<3, true>(p, n_ctas, stream) : launch_ws_pdf<3, false>(p, n_ctas, stream);
+	if (n_pos_dims == 2) return train ? launch_ws_pdf<2, true>(p, n_ctas, stream) : launch_ws_pdf<2, false>(p, n_ctas, stream);
 	return cudaErrorInvalidValue;
 }
 

@@ -201,7 +201,8 @@ __global__ void mlp_grad_finalize_kernel(uint32_t n, float* __restrict__ dw_accu
 // dL/d(output) rows (x loss_scale, through the output activation's transfer, padding columns zero), per-element values, sum.
 // Same expressions as the fused kernel's output epilogue (fused_common.cuh loss_element).
 __global__ void loss_kernel(uint32_t loss_type, uint32_t out_act, uint32_t batch, uint32_t n_out, uint32_t stride, float loss_scale, float n_total, const __half* __restrict__ prediction,
-                            const float* __restrict__ targets, __half* __restrict__ dL_dy, float* __restrict__ loss_values, float* __restrict__ loss_sum) {
+                            const float* __restrict__ targets, const float* __restrict__ data_pdf, __half* __restrict__ dL_dy, float* __restrict__ loss_values,
+                            float* __restrict__ loss_sum) {
 	pdl_wait();
 	pdl_launch_dependents();
 	// one thread per (sample, group of 8 output columns): 16-byte loads / stores of the fp16 rows
@@ -220,7 +221,9 @@ __global__ void loss_kernel(uint32_t loss_type, uint32_t out_act, uint32_t batch
 			float gq = 0.0f;
 			if (q < n_out) {
 				float value, grad;
-				fused::loss_element(loss_type, __half2float(y[k]), targets[(size_t)sample * n_out + q], n_total, luminance, value, grad);
+				const size_t t = (size_t)sample * n_out + q;
+				if (data_pdf) fused::loss_element_pdf(loss_type, __half2float(y[k]), targets[t], data_pdf[t], n_total, luminance, value, grad);
+				else fused::loss_element(loss_type, __half2float(y[k]), targets[t], n_total, luminance, value, grad);
 				gq = loss_scale * grad / n_total;
 				value_sum += value;
 				if (loss_values) loss_values[(size_t)sample * n_out + q] = value;
@@ -405,10 +408,10 @@ cudaError_t launch_mlp_grad_finalize(cudaStream_t stream, uint32_t n, float* dw_
 }
 
 cudaError_t launch_loss(cudaStream_t stream, uint32_t loss_type, uint32_t output_activation, uint32_t batch, uint32_t n_out, uint32_t stride, float loss_scale, uint32_t n_total,
-                        const __half* prediction, const float* targets, __half* dL_dy, float* loss_values, float* loss_sum) {
+                        const __half* prediction, const float* targets, const float* data_pdf, __half* dL_dy, float* loss_values, float* loss_sum) {
 	if ((uint64_t)batch * stride >= (1ull << 32) || stride % 8 != 0) return cudaErrorInvalidValue;
 	return launch_pdl(loss_kernel, blocks_for(batch * (stride / 8), 256), 256, 0, stream, loss_type, output_activation, batch, n_out, stride, loss_scale, (float)n_total, prediction, targets,
-	                  dL_dy, loss_values, loss_sum);
+	                  data_pdf, dL_dy, loss_values, loss_sum);
 }
 
 cudaError_t launch_activation_backward_output(cudaStream_t stream, uint32_t activation, uint64_t n, const __half* grad, const __half* forward_output, __half* out) {

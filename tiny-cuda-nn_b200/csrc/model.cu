@@ -148,7 +148,8 @@ struct Model {
 	DeviceBuffer<long long> dbg_clock;  // TCNNB_CLOCKS=<file> in ablation builds: phase stamps of the last ws launch
 	FusedStepParams fused{};                // the fused kernel's per-model arguments (configurations it runs); make_params adds the per-call ones
 	DeviceBuffer<__half> denc_scratch;      // module tier: dL/d(encoded) rows [n][64] handed from the fused kernel to the input-gradient kernel
-	DeviceBuffer<__half> grads_scratch;     // module tier: gradient array when the caller wants dL/d(input) only
+	DeviceBuffer<__half> grads_scratch;     // module tier: gradient array when the caller wants dL/d(input) only; trainer: GradientMode::Ignore / Accumulate
+	DeviceBuffer<float> dw_scratch;         // trainer, GradientMode::Ignore: network weight-gradient sums nobody reads
 	bool mlp_grads_in_accum = false;
 	// General (unfused) path: configurations the fused kernel does not cover -- 128 neurons, n_features_per_level in {1, 4, 8}, 4-D
 	// inputs, Nearest interpolation, wider encodings / outputs -- run as encoding kernel -> stand-alone MLP kernels -> encoding backward
@@ -517,13 +518,14 @@ static void general_forward(Model& m, cudaStream_t stream, uint32_t batch, const
 }
 
 // Forward + loss (or the caller's dL/d(output)) + backward on the general path. Gradients land where the fused kernel leaves them:
-// fp32 network weight-gradient sums in dw_accum, fp16 table gradients in grads + n_mlp_params. `dL_dinput` (fp32 [batch][n_in]) optional.
+// fp32 network weight-gradient sums in dw_accum, fp16 table gradients in grads + n_mlp_params (overwritten). `dL_dinput` (fp32
+// [batch][n_in]) and `data_pdf` optional; `keep_mlp_accum`: add onto the fp32 sums a previous step left (GradientMode::Accumulate).
 static void general_backward_pass(Model& m, cudaStream_t stream, uint32_t batch, uint32_t loss_batch, const float* x, const float* y, const __half* params, __half* grads,
-                                  const __half* ext_dL_doutput, float* dL_dinput, bool want_param_grads) {
+                                  const __half* ext_dL_doutput, float* dL_dinput, bool want_param_grads, const float* data_pdf = nullptr, bool keep_mlp_accum = false) {
 	const MlpConfig& mlp = m.mlp;
 	const bool grid_params = m.plan.n_params != 0 && want_param_grads;
 	if (!ext_dL_doutput) TCNNB_CUDA_CHECK(cudaMemsetAsync(m.scalars.ptr, 0, sizeof(float), stream));
-	if (m.mlp_grads_in_accum) {
+	if (m.mlp_grads_in_accum && !keep_mlp_accum) {
 		TCNNB_CUDA_CHECK(cudaMemsetAsync(m.dw_accum.ptr, 0, sizeof(float) * mlp.n_params, stream));
 		m.mlp_grads_in_accum = false;
 	}
@@ -539,10 +541,11 @@ static void general_backward_pass(Model& m, cudaStream_t stream, uint32_t batch,
 	const __half* dL_doutput = ext_dL_doutput;
 	if (!ext_dL_doutput) {
 		grow(m.g_dy, (size_t)batch * mlp.padded_out_width);
-		TCNNB_CUDA_CHECK(launch_loss(stream, m.loss_type, mlp.output_activation, batch, m.n_out, mlp.padded_out_width, m.loss_scale, loss_batch * m.n_out, out_rows, y, m.g_dy.ptr,
-		                             m.taps.loss_values, m.scalars.ptr));
+		__half* const dy_rows = (m.taps.dL_doutput && mlp.padded_out_width == 16) ? (__half*)m.taps.dL_doutput : m.g_dy.ptr;
+		TCNNB_CUDA_CHECK(launch_loss(stream, m.loss_type, mlp.output_activation, batch, m.n_out, mlp.padded_out_width, m.loss_scale, loss_batch * m.n_out, out_rows, y, data_pdf,
+		                             dy_rows, m.taps.loss_values, m.scalars.ptr));
 		++g_kernel_launches;
-		dL_doutput = m.g_dy.ptr;
+		dL_doutput = dy_rows;
 	}
 	const bool need_denc = grid_params || dL_dinput;
 	if (need_denc) grow(m.g_denc, (size_t)batch * mlp.in_width);
@@ -557,12 +560,16 @@ static void general_backward_pass(Model& m, cudaStream_t stream, uint32_t batch,
 
 // `targets_ready`: optional event the fused kernel (the first consumer of `y`) waits for; everything before it in the step --
 // gradient zeroing, the binning pass -- only needs `x` and runs while the targets are still in flight.
-// Caller-owned arrays of the module tier (cpp_api.h:76-104): working-precision parameters, gradient array, dL/d(output).
+// Arrays of a fused step other than the trainer's own: the module tier's caller-owned ones (cpp_api.h:76-104) and the optional arguments
+// of Trainer::training_step (tcnnb_training_step_ex).
 struct ModuleIO {
 	const __half* params = nullptr;
 	__half* grads = nullptr;
-	const __half* dL_doutput = nullptr;
+	const __half* dL_doutput = nullptr;  // optional: replaces the loss (targets unused)
 	__half* dL_dencoded = nullptr;  // optional [n][64] fp16: the network's input gradient rows, for the input-position gradient
+	const float* data_pdf = nullptr;  // optional [n][n_out]: the loss divides by it
+	float* dw_accum = nullptr;        // optional: fp32 network weight-gradient sums other than the model's (GradientMode::Ignore)
+	bool accumulate = false;          // add onto `grads` and the fp32 sums instead of overwriting them (GradientMode::Accumulate / Ignore)
 };
 
 static void training_step(Model& m, cudaStream_t stream, uint32_t batch, uint32_t loss_batch, const float* x, const float* y, bool run_optimizer, cudaEvent_t targets_ready = nullptr,
@@ -578,17 +585,19 @@ static void training_step(Model& m, cudaStream_t stream, uint32_t batch, uint32_
 		return;
 	}
 	__half* const grads_base = io ? io->grads : m.grads_fp16;
+	float* const dw_accum = io && io->dw_accum ? io->dw_accum : m.dw_accum.ptr;
+	const bool overwrite = !(io && io->accumulate);
 	// GradientMode::Overwrite: zero the grid gradient table (grid.h:865-867) and the loss accumulator -- inside the binning pass
-	// when there is one, else as memsets.
+	// when there is one, else as memsets. Accumulate zeroes the loss accumulator only.
 	__half* const grid_grads = grads_base + m.mlp.n_params;
 	const size_t grid_grad_bytes = sizeof(__half) * m.plan.n_params;
 	const bool bin = m.binning && batch >= 16384 && single_encoding(m.plan, FEAT_GRID);  // spatial order only matters to the table gathers
-	const bool zero_in_binning = bin && (((uintptr_t)grid_grads | grid_grad_bytes) & 15u) == 0;
+	const bool zero_in_binning = overwrite && bin && (((uintptr_t)grid_grads | grid_grad_bytes) & 15u) == 0;
 	if (!zero_in_binning) {
-		TCNNB_CUDA_CHECK(cudaMemsetAsync(grid_grads, 0, grid_grad_bytes, stream));
+		if (overwrite) TCNNB_CUDA_CHECK(cudaMemsetAsync(grid_grads, 0, grid_grad_bytes, stream));
 		TCNNB_CUDA_CHECK(cudaMemsetAsync(m.scalars.ptr, 0, sizeof(float), stream));
 	}
-	if (m.mlp_grads_in_accum) {
+	if (overwrite && m.mlp_grads_in_accum) {
 		// a previous step left un-consumed weight gradients (run_optimizer == false twice in a row): Overwrite semantics
 		TCNNB_CUDA_CHECK(cudaMemsetAsync(m.dw_accum.ptr, 0, sizeof(float) * m.mlp.n_params, stream));
 	}
@@ -596,11 +605,15 @@ static void training_step(Model& m, cudaStream_t stream, uint32_t batch, uint32_
 	if (io) {
 		p.params = io->params;
 		p.grads = io->grads;
-		p.ext_dy = io->dL_doutput;
+		p.dw_accum = dw_accum;
+		p.data_pdf = io->data_pdf;
 		if (io->dL_dencoded) p.dbg_denc = io->dL_dencoded;
-		p.targets = nullptr;
-		p.loss_sum = nullptr;
-		p.loss_values = nullptr;
+		if (io->dL_doutput) {
+			p.ext_dy = io->dL_doutput;
+			p.targets = nullptr;
+			p.loss_sum = nullptr;
+			p.loss_values = nullptr;
+		}
 	}
 	m.prof_mark(stream);
 	// Process the batch in (y, z)-column order: same sums, far fewer distinct memory sectors on the coarse levels (binning.cu).
@@ -628,7 +641,7 @@ static void training_step(Model& m, cudaStream_t stream, uint32_t batch, uint32_
 	++g_kernel_launches;
 	m.last_stream = stream;
 	m.prof_mark(stream);
-	m.mlp_grads_in_accum = true;
+	if (dw_accum == m.dw_accum.ptr) m.mlp_grads_in_accum = true;
 	if (run_optimizer) {
 		optimizer_step(m, stream);
 	}
@@ -924,6 +937,77 @@ __global__ void half_to_float_kernel(uint64_t n, const __half* __restrict__ in, 
 	const uint64_t i = threadIdx.x + (uint64_t)blockIdx.x * blockDim.x;
 	if (i < n) out[i] = (float)in[i];
 }
+
+__global__ void half_accumulate_kernel(uint64_t n, const __half* __restrict__ in, __half* __restrict__ inout) {
+	const uint64_t i = threadIdx.x + (uint64_t)blockIdx.x * blockDim.x;
+	if (i < n) inout[i] = __hadd(inout[i], in[i]);
+}
+
+// tcnn::GradientMode (object.h:116-120)
+enum GradientMode : int { GRADIENT_IGNORE = 0, GRADIENT_OVERWRITE = 1, GRADIENT_ACCUMULATE = 2 };
+
+// Trainer::training_step with all of its arguments (trainer.h:254-357): the fused kernel or the general path with the loss weighted by
+// `data_pdf`, or with the caller's `ext_dL_dy` (fp16 [batch][padded_output_width], already x loss scale) in place of the loss; the
+// gradients overwrite, add onto or leave alone the trainer's buffer; `dL_dinput` (fp32 [batch][n_in]) is overwritten. The optimizer
+// step, when asked for, comes last: the input gradient reads the parameters the step used.
+static void training_step_ex(Model& m, cudaStream_t stream, uint32_t batch, const float* x, const float* y, const float* data_pdf, bool run_optimizer, float* dL_dinput,
+                             bool use_inference_params, int mode, const __half* ext_dL_dy) {
+	if (m.module_only) throw std::runtime_error("this handle was created with tcnnb_module_create: use the tcnnb_module_* calls.");
+	if (m.dp) throw std::runtime_error("training_step_ex: data-parallel handles train with tcnnb_dp_training_step.");
+	if (mode != GRADIENT_IGNORE && mode != GRADIENT_OVERWRITE && mode != GRADIENT_ACCUMULATE) {
+		throw std::runtime_error("training_step_ex: param_gradients_mode must be 0 (Ignore), 1 (Overwrite) or 2 (Accumulate).");
+	}
+	if (!ext_dL_dy && !y) throw std::runtime_error("training_step: target is null and no external_dL_dy replaces the loss.");
+	if (!x) throw std::runtime_error("training_step: input is null.");
+	check_batch(batch);
+	if (ext_dL_dy) data_pdf = nullptr;  // the loss is not evaluated (trainer.h:127-131)
+	const __half* params = use_inference_params ? m.inference_params() : m.params_fp16;
+	const uint32_t n_mlp = m.mlp.n_params;
+	if (mode == GRADIENT_ACCUMULATE && !m.mlp_grads_in_accum && n_mlp) {
+		// the network's gradients are the fp16 values in the buffer (tcnnb_param_gradients materialised them): the fp32 sums continue
+		// from there
+		half_to_float_kernel<<<(n_mlp + 255) / 256, 256, 0, stream>>>(n_mlp, m.grads_fp16, m.dw_accum.ptr);
+		TCNNB_CUDA_CHECK(cudaGetLastError());
+		++g_kernel_launches;
+		m.mlp_grads_in_accum = true;
+	}
+	if (mode != GRADIENT_OVERWRITE) m.grads_scratch.resize(m.n_params_padded);
+	if (m.use_general()) {
+		if (ext_dL_dy) TCNNB_CUDA_CHECK(cudaMemsetAsync(m.scalars.ptr, 0, sizeof(float), stream));
+		// the general path overwrites the table gradients it computes: Accumulate adds them onto the buffer afterwards
+		__half* const grads = mode == GRADIENT_OVERWRITE ? m.grads_fp16 : m.grads_scratch.ptr;
+		general_backward_pass(m, stream, batch, batch, x, y, params, grads, ext_dL_dy, dL_dinput, mode != GRADIENT_IGNORE, data_pdf, mode != GRADIENT_OVERWRITE);
+		if (mode == GRADIENT_ACCUMULATE && m.plan.n_params) {
+			half_accumulate_kernel<<<(uint32_t)((m.plan.n_params + 255) / 256), 256, 0, stream>>>(m.plan.n_params, grads + n_mlp, m.grads_fp16 + n_mlp);
+			TCNNB_CUDA_CHECK(cudaGetLastError());
+			++g_kernel_launches;
+		}
+	} else {
+		if (dL_dinput && single_encoding(m.plan, FEAT_IDENTITY)) {
+			throw std::runtime_error("training_step: input gradients through an Identity encoding are not built for configurations the fused kernel runs; the general path (e.g. n_neurons > 64) computes them.");
+		}
+		ModuleIO io;
+		io.params = params;
+		io.dL_doutput = ext_dL_dy;
+		io.data_pdf = data_pdf;
+		io.accumulate = mode != GRADIENT_OVERWRITE;
+		io.grads = m.grads_fp16;
+		if (mode == GRADIENT_IGNORE) {
+			// the kernel still scatters: into scratch (trainer.h:338 hands the reference's a null gradient buffer). The scratch is never
+			// zeroed, so its sums keep growing over Ignore steps; nothing reads it.
+			io.grads = m.grads_scratch.ptr;
+			m.dw_scratch.resize(n_mlp);
+			io.dw_accum = m.dw_scratch.ptr;
+		}
+		if (dL_dinput) {
+			m.denc_scratch.resize(std::max(m.denc_scratch.n, (size_t)batch * 64));
+			io.dL_dencoded = m.denc_scratch.ptr;
+		}
+		training_step(m, stream, batch, batch, x, y, false, nullptr, &io);
+		if (dL_dinput) plan_input_gradient(m.plan, stream, batch, x, params + n_mlp, m.denc_scratch.ptr, 64, dL_dinput, 1.0f);
+	}
+	if (run_optimizer) optimizer_step(m, stream);
+}
 }  // namespace tcnnb
 
 
@@ -1082,6 +1166,14 @@ int tcnnb_set_optimizer_progress(tcnnb_model* m, uint32_t current_step, float ba
 int tcnnb_training_step(tcnnb_model* m, tcnnb_stream stream, uint32_t batch_size, const float* input_dev, const float* target_dev, int run_optimizer) {
 	TCNNB_API_BEGIN
 	training_step(m->impl, (cudaStream_t)stream, batch_size, batch_size, input_dev, target_dev, run_optimizer != 0);
+	TCNNB_API_END
+}
+
+int tcnnb_training_step_ex(tcnnb_model* m, tcnnb_stream stream, uint32_t batch_size, const float* input_dev, const float* target_dev, const float* data_pdf_dev, int run_optimizer,
+                           float* dL_dinput_dev, int use_inference_params, int param_gradients_mode, const void* external_dL_dy_dev) {
+	TCNNB_API_BEGIN
+	training_step_ex(m->impl, (cudaStream_t)stream, batch_size, input_dev, target_dev, data_pdf_dev, run_optimizer != 0, dL_dinput_dev, use_inference_params != 0, param_gradients_mode,
+	                 (const __half*)external_dL_dy_dev);
 	TCNNB_API_END
 }
 

@@ -61,6 +61,7 @@ ABI = [
     ("tcnnb_optimizer_state", _int, [_vp, ctypes.POINTER(_vp), ctypes.POINTER(_vp), ctypes.POINTER(_vp), ctypes.POINTER(_u32), _f32p]),
     ("tcnnb_set_optimizer_progress", _int, [_vp, _u32, ctypes.c_float]),
     ("tcnnb_training_step", _int, [_vp, _vp, _u32, _vp, _vp, _int]),
+    ("tcnnb_training_step_ex", _int, [_vp, _vp, _u32, _vp, _vp, _vp, _int, _vp, _int, _int, _vp]),
     ("tcnnb_training_step_shard", _int, [_vp, _vp, _u32, _u32, _vp, _vp, _int]),
     ("tcnnb_optimizer_step", _int, [_vp, _vp]),
     ("tcnnb_generate_random_uniform", _int, [_vp, ctypes.c_uint64, ctypes.c_uint64, ctypes.c_uint64, _vp, ctypes.c_float, ctypes.c_float]),
@@ -194,13 +195,38 @@ class _Trainer:
     def __init__(self, model):
         self._m = model
 
-    def training_step(self, inputs, targets, run_optimizer=True, stream=None):
+    _GRADIENT_MODES = {"Ignore": 0, "Overwrite": 1, "Accumulate": 2}
+
+    def training_step(self, inputs, targets, run_optimizer=True, stream=None, data_pdf=None, dL_dinput=None, use_inference_params=False,
+                      gradient_mode="Overwrite", external_dL_dy=None):
+        """trainer.training_step (trainer.h:254-357). `data_pdf` [B, n_out] fp32 divides the loss per element; `external_dL_dy`
+        [B, padded_output_width] fp16, already multiplied by the loss scale, replaces the loss (targets may then be None);
+        `dL_dinput` [B, n_in] fp32 is overwritten with dL/d(input); `gradient_mode` is "Ignore", "Overwrite" or "Accumulate"."""
         import torch
 
         m = self._m
-        assert inputs.is_cuda and targets.is_cuda and inputs.dtype == torch.float32 and targets.dtype == torch.float32
-        assert inputs.is_contiguous() and targets.is_contiguous()
-        _check(load().tcnnb_training_step(m._h, _stream_handle(stream), inputs.shape[0], inputs.data_ptr(), targets.data_ptr(), int(run_optimizer)))
+        assert inputs.is_cuda and inputs.dtype == torch.float32 and inputs.is_contiguous()
+        extras = data_pdf is not None or dL_dinput is not None or use_inference_params or gradient_mode != "Overwrite" or external_dL_dy is not None
+        if not extras:
+            assert targets.is_cuda and targets.dtype == torch.float32 and targets.is_contiguous()
+            _check(load().tcnnb_training_step(m._h, _stream_handle(stream), inputs.shape[0], inputs.data_ptr(), targets.data_ptr(), int(run_optimizer)))
+            return self
+        if gradient_mode not in self._GRADIENT_MODES:
+            raise ValueError(f"gradient_mode must be one of {sorted(self._GRADIENT_MODES)}, not {gradient_mode!r}")
+        B = inputs.shape[0]
+
+        def ptr(t, dtype, shape):
+            if t is None:
+                return None
+            if not (t.is_cuda and t.dtype == dtype and t.is_contiguous() and tuple(t.shape) == shape):
+                raise ValueError(f"expected a contiguous CUDA {dtype} tensor of shape {shape}, got {t.dtype} {tuple(t.shape)}")
+            return t.data_ptr()
+
+        lib = load()
+        n_out, pad = m.n_output_dims, lib.tcnnb_padded_output_width(m._h)
+        _check(lib.tcnnb_training_step_ex(m._h, _stream_handle(stream), B, inputs.data_ptr(), ptr(targets, torch.float32, (B, n_out)),
+                                          ptr(data_pdf, torch.float32, (B, n_out)), int(run_optimizer), ptr(dL_dinput, torch.float32, (B, m.n_input_dims)),
+                                          int(bool(use_inference_params)), self._GRADIENT_MODES[gradient_mode], ptr(external_dL_dy, torch.float16, (B, pad))))
         return self
 
     def training_step_shard(self, inputs, targets, global_batch_size, run_optimizer=False, stream=None):
