@@ -299,7 +299,8 @@ typedef struct {
 } tcnnb_debug_taps;
 int tcnnb_set_debug_taps(tcnnb_model* m, const tcnnb_debug_taps* taps);
 /* Test-only switches (not dispatch knobs of the product path): "binning" 0/1 -- run the step without / with the spatial
- * binning pass (tests assert both touch the same table entries). */
+ * binning pass (tests assert both touch the same table entries); "adam_steps32" 1 -- keep Adam's step counters 32 bits wide
+ * although 16-bit ones give the same updates (tests compare the two layouts), 0 -- back to the width the trainer chose. */
 int tcnnb_debug_set(tcnnb_model* m, const char* key, int value);
 /* Per-kernel device timing for the roofline report: when enabled, CUDA events bracket the binning kernels, the fused fwd+bwd kernel
  * and the optimizer kernel of every training step on the caller's stream; tcnnb_read_profile synchronises and returns the sums. */

@@ -79,9 +79,12 @@ __global__ void level_scales_kernel(uint32_t n_levels, float log2_per_level_scal
 //     for API visibility, and the accumulator is re-armed to zero for the next step.
 //   * optimizer state streams use evict-first loads/stores so that the fp16 table + gradient table stay L2 resident.
 // ------------------------------------------------------------------------------------------------------------------
-// One Adam update, shared by the scalar and the 4-wide kernels. Returns false if the parameter is skipped.
+// One Adam update, shared by every Adam kernel. Returns false if the parameter is skipped. `Step` is the per-parameter counter:
+// uint32_t, or uint16_t saturating at 65535 -- exact when adam_u16_steps_exact() holds, because from t = 65535 on the bias
+// correction below is exactly 1 for every larger t.
+template <typename Step>
 __device__ __forceinline__ bool adam_update(const AdamParams& a, const bool is_matrix, const float loss_scale, const __half grad_h,
-                                            float& weight_fp, float& first_moment, float& second_moment, uint32_t& step) {
+                                            float& weight_fp, float& first_moment, float& second_moment, Step& step) {
 	float gradient = (float)grad_h / loss_scale;
 	if (!is_matrix) {
 		if (!a.optimize_non_matrix_params || (gradient == 0 && a.skip_zero_grad_non_matrix_params)) return false;
@@ -101,7 +104,12 @@ __device__ __forceinline__ bool adam_update(const AdamParams& a, const bool is_m
 	second_moment = a.beta2 * second_moment + (1 - a.beta2) * gradient_sq;
 	float learning_rate = a.learning_rate;
 	if (!is_matrix) learning_rate *= a.non_matrix_learning_rate_factor;
-	const uint32_t current_step = ++step;
+	if constexpr (sizeof(Step) == 2) {
+		step = step == 0xFFFFu ? step : (Step)(step + 1);
+	} else {
+		++step;
+	}
+	const uint32_t current_step = step;
 	learning_rate *= sqrtf(1 - powf(a.beta2, (float)current_step)) / (1 - powf(a.beta1, (float)current_step));
 	const float effective_learning_rate = fminf(fmaxf(learning_rate / (sqrtf(second_moment) + a.epsilon), a.lower_lr_bound), a.upper_lr_bound);
 	const float decayed_weight = (1 - a.relative_decay * learning_rate) * weight_fp - copysignf(a.absolute_decay * learning_rate, weight_fp);
@@ -114,11 +122,12 @@ __device__ __forceinline__ bool adam_update(const AdamParams& a, const bool is_m
 }
 
 // One parameter per thread: the tail / unaligned path (caller-provided arrays that are not 16-byte aligned, lengths that are not a
-// multiple of four); same update as the 4-wide kernel.
+// multiple of eight); same update as the 8-wide kernel.
+template <typename Step>
 __global__ void adam_step_kernel(const AdamParams a, const uint32_t n_elements, const uint32_t n_matrix_weights, const float loss_scale,
                                  float* __restrict__ weights_full_precision, __half* __restrict__ weights, __half* __restrict__ gradients,
                                  float* __restrict__ dw_accum, float* __restrict__ first_moments, float* __restrict__ second_moments,
-                                 uint32_t* __restrict__ param_steps) {
+                                 Step* __restrict__ param_steps) {
 	pdl_wait();  // no early pdl_launch_dependents(): a long bandwidth-bound kernel should not share its SMs with parked CTAs
 	const uint32_t i = threadIdx.x + blockIdx.x * blockDim.x;
 	if (i >= n_elements) return;
@@ -131,7 +140,7 @@ __global__ void adam_step_kernel(const AdamParams a, const uint32_t n_elements, 
 		grad_h = gradients[i];
 	}
 	float w = __ldcs(weights_full_precision + i), m = __ldcs(first_moments + i), v = __ldcs(second_moments + i);
-	uint32_t st = __ldcs(param_steps + i);
+	Step st = __ldcs(param_steps + i);
 	if (!adam_update(a, i < n_matrix_weights, loss_scale, grad_h, w, m, v, st)) return;
 	__stcs(weights_full_precision + i, w);
 	__stcs(first_moments + i, m);
@@ -140,51 +149,90 @@ __global__ void adam_step_kernel(const AdamParams a, const uint32_t n_elements, 
 	weights[i] = (__half)w;
 }
 
-// 4 parameters per thread: 128-bit streaming accesses to the fp32 state, 64-bit to the fp16 params / gradients.
-// Groups whose four gradients are all zero (untouched hash-table entries) touch nothing but the 8 gradient bytes.
-__global__ void __launch_bounds__(256) adam_step_vec4_kernel(const AdamParams a, const uint32_t n_groups, const uint32_t n_matrix_weights, const float loss_scale,
-                                      float4* __restrict__ weights_full_precision, uint2* __restrict__ weights, uint2* __restrict__ gradients,
+// 8 parameters per thread, every access 128 bits wide: two float4 of each fp32 stream, one uint4 of fp16 params / gradients, and
+// one (uint16_t) or two (uint32_t) uint4 of step counters. Groups whose eight gradients are all zero (untouched hash-table entries)
+// write nothing back.
+template <typename Step>
+__global__ void __launch_bounds__(256) adam_step_vec8_kernel(const AdamParams a, const uint32_t n_groups, const uint32_t n_matrix_weights, const float loss_scale,
+                                      float4* __restrict__ weights_full_precision, uint4* __restrict__ weights, uint4* __restrict__ gradients,
                                       float4* __restrict__ dw_accum, float4* __restrict__ first_moments, float4* __restrict__ second_moments,
                                       uint4* __restrict__ param_steps) {
+	constexpr uint32_t S = sizeof(Step) / 2;  // uint4 chunks of step counters per group
 	pdl_wait();
 	const uint32_t gidx = threadIdx.x + blockIdx.x * blockDim.x;
 	if (gidx >= n_groups) return;
-	const uint32_t i0 = gidx * 4;
+	const uint32_t i0 = gidx * 8;
 
 	// Issue every load of this group up front (independent 128-bit streams); the zero-gradient early-out below only
 	// saves the write-back -- untouched groups are ~2 % of a step, memory-level parallelism matters more.
-	const bool from_accum = i0 + 3 < n_matrix_weights && dw_accum != nullptr;
-	const uint2 raw = from_accum ? make_uint2(0, 0) : gradients[gidx];
-	const float4 w4 = __ldcs(weights_full_precision + gidx);
-	const float4 m4 = __ldcs(first_moments + gidx);
-	const float4 v4 = __ldcs(second_moments + gidx);
-	const uint4 s4 = __ldcs(param_steps + gidx);
+	const bool from_accum = i0 + 7 < n_matrix_weights && dw_accum != nullptr;
+	const uint4 raw = from_accum ? make_uint4(0, 0, 0, 0) : gradients[gidx];
+	const float4 wa = __ldcs(weights_full_precision + 2 * gidx), wb = __ldcs(weights_full_precision + 2 * gidx + 1);
+	const float4 ma = __ldcs(first_moments + 2 * gidx), mb = __ldcs(first_moments + 2 * gidx + 1);
+	const float4 va = __ldcs(second_moments + 2 * gidx), vb = __ldcs(second_moments + 2 * gidx + 1);
+	union {
+		uint4 q[S];
+		Step s[8];
+	} st;
+#pragma unroll
+	for (uint32_t k = 0; k < S; ++k) st.q[k] = __ldcs(param_steps + S * gidx + k);
 
-	__half g[4];
+	union {
+		uint4 q;
+		__half h[8];
+	} g;
 	if (from_accum) {
-		const float4 acc = dw_accum[gidx];
-		dw_accum[gidx] = make_float4(0.f, 0.f, 0.f, 0.f);
-		g[0] = (__half)acc.x; g[1] = (__half)acc.y; g[2] = (__half)acc.z; g[3] = (__half)acc.w;
-		gradients[gidx] = *reinterpret_cast<const uint2*>(g);
+		const float4 acc0 = dw_accum[2 * gidx], acc1 = dw_accum[2 * gidx + 1];
+		dw_accum[2 * gidx] = make_float4(0.f, 0.f, 0.f, 0.f);
+		dw_accum[2 * gidx + 1] = make_float4(0.f, 0.f, 0.f, 0.f);
+		g.h[0] = (__half)acc0.x; g.h[1] = (__half)acc0.y; g.h[2] = (__half)acc0.z; g.h[3] = (__half)acc0.w;
+		g.h[4] = (__half)acc1.x; g.h[5] = (__half)acc1.y; g.h[6] = (__half)acc1.z; g.h[7] = (__half)acc1.w;
+		gradients[gidx] = g.q;
 	} else {
-		*reinterpret_cast<uint2*>(g) = raw;
-		if (i0 >= n_matrix_weights && a.skip_zero_grad_non_matrix_params && ((raw.x | raw.y) & 0x7FFF7FFFu) == 0) return;  // all four are +-0
+		g.q = raw;
+		if (i0 >= n_matrix_weights && a.skip_zero_grad_non_matrix_params && ((raw.x | raw.y | raw.z | raw.w) & 0x7FFF7FFFu) == 0) return;  // all eight are +-0
 	}
 
-	float w[4] = {w4.x, w4.y, w4.z, w4.w}, m[4] = {m4.x, m4.y, m4.z, m4.w}, v[4] = {v4.x, v4.y, v4.z, v4.w};
-	uint32_t st[4] = {s4.x, s4.y, s4.z, s4.w};
+	float w[8] = {wa.x, wa.y, wa.z, wa.w, wb.x, wb.y, wb.z, wb.w}, m[8] = {ma.x, ma.y, ma.z, ma.w, mb.x, mb.y, mb.z, mb.w}, v[8] = {va.x, va.y, va.z, va.w, vb.x, vb.y, vb.z, vb.w};
 	bool any = false;
 #pragma unroll
-	for (uint32_t k = 0; k < 4; ++k) {
-		any |= adam_update(a, i0 + k < n_matrix_weights, loss_scale, g[k], w[k], m[k], v[k], st[k]);
+	for (uint32_t k = 0; k < 8; ++k) {
+		any |= adam_update(a, i0 + k < n_matrix_weights, loss_scale, g.h[k], w[k], m[k], v[k], st.s[k]);
 	}
 	if (!any) return;
-	__stcs(weights_full_precision + gidx, make_float4(w[0], w[1], w[2], w[3]));
-	__stcs(first_moments + gidx, make_float4(m[0], m[1], m[2], m[3]));
-	__stcs(second_moments + gidx, make_float4(v[0], v[1], v[2], v[3]));
-	__stcs(param_steps + gidx, make_uint4(st[0], st[1], st[2], st[3]));
-	__half h[4] = {(__half)w[0], (__half)w[1], (__half)w[2], (__half)w[3]};
-	weights[gidx] = *reinterpret_cast<const uint2*>(h);
+	__stcs(weights_full_precision + 2 * gidx, make_float4(w[0], w[1], w[2], w[3]));
+	__stcs(weights_full_precision + 2 * gidx + 1, make_float4(w[4], w[5], w[6], w[7]));
+	__stcs(first_moments + 2 * gidx, make_float4(m[0], m[1], m[2], m[3]));
+	__stcs(first_moments + 2 * gidx + 1, make_float4(m[4], m[5], m[6], m[7]));
+	__stcs(second_moments + 2 * gidx, make_float4(v[0], v[1], v[2], v[3]));
+	__stcs(second_moments + 2 * gidx + 1, make_float4(v[4], v[5], v[6], v[7]));
+#pragma unroll
+	for (uint32_t k = 0; k < S; ++k) __stcs(param_steps + S * gidx + k, st.q[k]);
+	union {
+		uint4 q;
+		__half h[8];
+	} h;
+#pragma unroll
+	for (uint32_t k = 0; k < 8; ++k) h.h[k] = (__half)w[k];
+	weights[gidx] = h.q;
+}
+
+// One thread: whether 1 - powf(beta, t) is exactly 1.0f for both betas at t = 65535 and at the largest 32-bit count, with the
+// device's own (fast-math) powf. powf(beta, t) is monotone in t, so every t in between gives the same bias correction, 1.
+__global__ void adam_u16_steps_exact_kernel(float beta1, float beta2, uint32_t* out) {
+	bool exact = true;
+	for (const float t : {65535.0f, 4294967295.0f}) exact = exact && 1 - powf(beta1, t) == 1.0f && 1 - powf(beta2, t) == 1.0f;
+	*out = exact;
+}
+
+__global__ void widen_steps_kernel(uint64_t n, const uint16_t* __restrict__ in, uint32_t* __restrict__ out) {
+	const uint64_t i = threadIdx.x + (uint64_t)blockIdx.x * blockDim.x;
+	if (i < n) out[i] = in[i];
+}
+
+__global__ void narrow_steps_kernel(uint64_t n, const uint32_t* __restrict__ in, uint16_t* __restrict__ out) {
+	const uint64_t i = threadIdx.x + (uint64_t)blockIdx.x * blockDim.x;
+	if (i < n) out[i] = (uint16_t)min(in[i], 0xFFFFu);
 }
 
 __global__ void mlp_grad_finalize_kernel(uint32_t n, float* __restrict__ dw_accum, __half* __restrict__ gradients) {
@@ -284,10 +332,11 @@ __global__ void dp_barrier_kernel(const DpPeers peers, const uint32_t epoch) {
 	}
 }
 
-template <bool MULTICAST>
+template <bool MULTICAST, typename Step>
 __global__ void __launch_bounds__(256) adam_step_dp_kernel(const AdamParams a, const DpPeers peers, const uint64_t first, const uint32_t n_groups, const uint32_t n_matrix_weights,
                                                             const uint64_t n_params, const float loss_scale, float* __restrict__ weights_full_precision,
-                                                            float* __restrict__ first_moments, float* __restrict__ second_moments, uint32_t* __restrict__ param_steps) {
+                                                            float* __restrict__ first_moments, float* __restrict__ second_moments, Step* __restrict__ param_steps) {
+	constexpr uint32_t S = sizeof(Step) / 2;  // uint4 chunks of step counters per group of 8
 	const uint32_t gidx = threadIdx.x + blockIdx.x * blockDim.x;
 	if (gidx >= n_groups) return;
 	const uint64_t i0 = first + (uint64_t)gidx * 8;
@@ -322,28 +371,31 @@ __global__ void __launch_bounds__(256) adam_step_dp_kernel(const AdamParams a, c
 	const float4* w4p = reinterpret_cast<const float4*>(weights_full_precision + i0);
 	const float4* m4p = reinterpret_cast<const float4*>(first_moments + i0);
 	const float4* v4p = reinterpret_cast<const float4*>(second_moments + i0);
-	const uint4* s4p = reinterpret_cast<const uint4*>(param_steps + i0);
+	uint4* const s4p = reinterpret_cast<uint4*>(param_steps + i0);
 	const float4 wa = __ldcs(w4p), wb = __ldcs(w4p + 1), ma = __ldcs(m4p), mb = __ldcs(m4p + 1), va = __ldcs(v4p), vb = __ldcs(v4p + 1);
-	const uint4 sa = __ldcs(s4p), sb = __ldcs(s4p + 1);
+	union {
+		uint4 q[S];
+		Step s[8];
+	} st;
+#pragma unroll
+	for (uint32_t k = 0; k < S; ++k) st.q[k] = __ldcs(s4p + k);
 	float w[8] = {wa.x, wa.y, wa.z, wa.w, wb.x, wb.y, wb.z, wb.w}, m[8] = {ma.x, ma.y, ma.z, ma.w, mb.x, mb.y, mb.z, mb.w}, v[8] = {va.x, va.y, va.z, va.w, vb.x, vb.y, vb.z, vb.w};
-	uint32_t st[8] = {sa.x, sa.y, sa.z, sa.w, sb.x, sb.y, sb.z, sb.w};
 	const __half* g = reinterpret_cast<const __half*>(gw);
 	bool any = false;
 #pragma unroll
-	for (uint32_t k = 0; k < 8; ++k) any |= adam_update(a, i0 + k < n_matrix_weights, loss_scale, g[k], w[k], m[k], v[k], st[k]);
+	for (uint32_t k = 0; k < 8; ++k) any |= adam_update(a, i0 + k < n_matrix_weights, loss_scale, g[k], w[k], m[k], v[k], st.s[k]);
 	if (!any) return;
 	float4* w4o = reinterpret_cast<float4*>(weights_full_precision + i0);
 	float4* m4o = reinterpret_cast<float4*>(first_moments + i0);
 	float4* v4o = reinterpret_cast<float4*>(second_moments + i0);
-	uint4* s4o = reinterpret_cast<uint4*>(param_steps + i0);
 	__stcs(w4o, make_float4(w[0], w[1], w[2], w[3]));
 	__stcs(w4o + 1, make_float4(w[4], w[5], w[6], w[7]));
 	__stcs(m4o, make_float4(m[0], m[1], m[2], m[3]));
 	__stcs(m4o + 1, make_float4(m[4], m[5], m[6], m[7]));
 	__stcs(v4o, make_float4(v[0], v[1], v[2], v[3]));
 	__stcs(v4o + 1, make_float4(v[4], v[5], v[6], v[7]));
-	__stcs(s4o, make_uint4(st[0], st[1], st[2], st[3]));
-	__stcs(s4o + 1, make_uint4(st[4], st[5], st[6], st[7]));
+#pragma unroll
+	for (uint32_t k = 0; k < S; ++k) __stcs(s4p + k, st.q[k]);
 	// ---- publish the working-precision weights to every replica
 	uint32_t hw[4];
 #pragma unroll
@@ -382,23 +434,49 @@ cudaError_t launch_level_scales(cudaStream_t stream, uint32_t n_levels, float lo
 	return cudaGetLastError();
 }
 
+template <typename Step>
 cudaError_t launch_adam_step(cudaStream_t stream, const AdamParams& a, uint32_t n_elements, uint32_t n_matrix_weights, float loss_scale,
                              float* weights_full_precision, __half* weights, __half* gradients, float* dw_accum, float* first_moments,
-                             float* second_moments, uint32_t* param_steps) {
+                             float* second_moments, Step* param_steps) {
 	if (n_elements == 0) return cudaSuccess;
 	auto aligned = [](const void* p, size_t a) { return ((uintptr_t)p % a) == 0; };
 	// A skipped lane of a partially updated group is written back with its loaded (unchanged) value, which is only
 	// equivalent to "not touched" if the weights' fp16 copy equals (half)fp32 master -- true for trainer-owned buffers.
-	const bool vec_ok = n_elements % 4 == 0 && n_matrix_weights % 4 == 0 && aligned(weights_full_precision, 16) && aligned(weights, 8) && aligned(gradients, 8) &&
+	const bool vec_ok = n_elements % 8 == 0 && n_matrix_weights % 8 == 0 && aligned(weights_full_precision, 16) && aligned(weights, 16) && aligned(gradients, 16) &&
 	                    aligned(first_moments, 16) && aligned(second_moments, 16) && aligned(param_steps, 16) && (dw_accum == nullptr || aligned(dw_accum, 16));
 	if (vec_ok) {
-		const uint32_t n_groups = n_elements / 4;
-		return launch_pdl(adam_step_vec4_kernel, blocks_for(n_groups, 256), 256, 0, stream, a, n_groups, n_matrix_weights, loss_scale, (float4*)weights_full_precision,
-		                  (uint2*)weights, (uint2*)gradients, (float4*)dw_accum, (float4*)first_moments, (float4*)second_moments, (uint4*)param_steps);
+		const uint32_t n_groups = n_elements / 8;
+		return launch_pdl(adam_step_vec8_kernel<Step>, blocks_for(n_groups, 256), 256, 0, stream, a, n_groups, n_matrix_weights, loss_scale, (float4*)weights_full_precision,
+		                  (uint4*)weights, (uint4*)gradients, (float4*)dw_accum, (float4*)first_moments, (float4*)second_moments, (uint4*)param_steps);
 	} else {
-		return launch_pdl(adam_step_kernel, blocks_for(n_elements, 256), 256, 0, stream, a, n_elements, n_matrix_weights, loss_scale, weights_full_precision, weights,
+		return launch_pdl(adam_step_kernel<Step>, blocks_for(n_elements, 256), 256, 0, stream, a, n_elements, n_matrix_weights, loss_scale, weights_full_precision, weights,
 		                  gradients, dw_accum, first_moments, second_moments, param_steps);
 	}
+}
+template cudaError_t launch_adam_step<uint16_t>(cudaStream_t, const AdamParams&, uint32_t, uint32_t, float, float*, __half*, __half*, float*, float*, float*, uint16_t*);
+template cudaError_t launch_adam_step<uint32_t>(cudaStream_t, const AdamParams&, uint32_t, uint32_t, float, float*, __half*, __half*, float*, float*, float*, uint32_t*);
+
+cudaError_t adam_u16_steps_exact(const AdamParams& a, bool* exact) {
+	uint32_t* flag = nullptr;
+	cudaError_t err = cudaMalloc(&flag, sizeof(uint32_t));
+	if (err != cudaSuccess) return err;
+	adam_u16_steps_exact_kernel<<<1, 1>>>(a.beta1, a.beta2, flag);
+	uint32_t value = 0;
+	err = cudaMemcpy(&value, flag, sizeof(uint32_t), cudaMemcpyDeviceToHost);
+	cudaFree(flag);
+	*exact = value != 0;
+	return err;
+}
+
+cudaError_t launch_widen_steps(cudaStream_t stream, uint64_t n, const uint16_t* in, uint32_t* out) {
+	if (n == 0) return cudaSuccess;
+	widen_steps_kernel<<<blocks_for(n, 256), 256, 0, stream>>>(n, in, out);
+	return cudaGetLastError();
+}
+
+cudaError_t launch_narrow_steps(cudaStream_t stream, uint64_t n, const uint32_t* in, uint16_t* out) {
+	if (n == 0) return cudaSuccess;
+	narrow_steps_kernel<<<blocks_for(n, 256), 256, 0, stream>>>(n, in, out);
 	return cudaGetLastError();
 }
 
@@ -430,19 +508,22 @@ cudaError_t launch_dp_barrier(cudaStream_t stream, const DpPeers& peers, uint32_
 	return cudaGetLastError();
 }
 
+template <typename Step>
 cudaError_t launch_adam_step_dp(cudaStream_t stream, const AdamParams& a, const DpPeers& peers, uint64_t first, uint64_t count, uint32_t n_matrix_weights, uint64_t n_params,
-                                float loss_scale, float* weights_full_precision, float* first_moments, float* second_moments, uint32_t* param_steps) {
+                                float loss_scale, float* weights_full_precision, float* first_moments, float* second_moments, Step* param_steps) {
 	if (count == 0) return cudaSuccess;
 	if (first % 8 != 0 || count % 8 != 0 || n_params % 8 != 0 || n_matrix_weights % 8 != 0) return cudaErrorInvalidValue;
 	const uint32_t n_groups = (uint32_t)(count / 8);
 	if (peers.grads_mc && peers.params_mc) {
-		adam_step_dp_kernel<true><<<blocks_for(n_groups, 256), 256, 0, stream>>>(a, peers, first, n_groups, n_matrix_weights, n_params, loss_scale, weights_full_precision, first_moments,
-		                                                                          second_moments, param_steps);
+		adam_step_dp_kernel<true, Step><<<blocks_for(n_groups, 256), 256, 0, stream>>>(a, peers, first, n_groups, n_matrix_weights, n_params, loss_scale, weights_full_precision, first_moments,
+		                                                                                second_moments, param_steps);
 	} else {
-		adam_step_dp_kernel<false><<<blocks_for(n_groups, 256), 256, 0, stream>>>(a, peers, first, n_groups, n_matrix_weights, n_params, loss_scale, weights_full_precision, first_moments,
-		                                                                           second_moments, param_steps);
+		adam_step_dp_kernel<false, Step><<<blocks_for(n_groups, 256), 256, 0, stream>>>(a, peers, first, n_groups, n_matrix_weights, n_params, loss_scale, weights_full_precision, first_moments,
+		                                                                                 second_moments, param_steps);
 	}
 	return cudaGetLastError();
 }
+template cudaError_t launch_adam_step_dp<uint16_t>(cudaStream_t, const AdamParams&, const DpPeers&, uint64_t, uint64_t, uint32_t, uint64_t, float, float*, float*, float*, uint16_t*);
+template cudaError_t launch_adam_step_dp<uint32_t>(cudaStream_t, const AdamParams&, const DpPeers&, uint64_t, uint64_t, uint32_t, uint64_t, float, float*, float*, float*, uint32_t*);
 
 }  // namespace tcnnb

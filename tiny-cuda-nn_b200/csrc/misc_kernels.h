@@ -28,9 +28,18 @@ struct AdamParams {
 cudaError_t launch_random_uniform(cudaStream_t stream, Pcg32 rng, uint64_t n_elements, float* out, float lower, float upper);
 cudaError_t launch_cast_params(cudaStream_t stream, uint64_t n, const float* in, __half* out);
 cudaError_t launch_level_scales(cudaStream_t stream, uint32_t n_levels, float log2_per_level_scale, uint32_t base_resolution, float* scales_dev);
+// Adam's per-parameter step counters are uint32_t, or uint16_t saturating at 65535 when adam_u16_steps_exact() says that this gives
+// bit-identical updates (Step = uint16_t or uint32_t).
+template <typename Step>
 cudaError_t launch_adam_step(cudaStream_t stream, const AdamParams& a, uint32_t n_elements, uint32_t n_matrix_weights, float loss_scale,
                              float* weights_full_precision, __half* weights, __half* gradients, float* dw_accum, float* first_moments,
-                             float* second_moments, uint32_t* param_steps);
+                             float* second_moments, Step* param_steps);
+// Whether Adam's bias correction sqrtf(1 - powf(beta2, t)) / (1 - powf(beta1, t)), evaluated on the device, is exactly 1 for every
+// t >= 65535: then a counter that stops at 65535 updates exactly like one that keeps counting. Synchronous (one-thread probe).
+cudaError_t adam_u16_steps_exact(const AdamParams& a, bool* exact);
+// uint16_t <-> uint32_t copies of the step counters (narrowing saturates at 65535).
+cudaError_t launch_widen_steps(cudaStream_t stream, uint64_t n, const uint16_t* in, uint32_t* out);
+cudaError_t launch_narrow_steps(cudaStream_t stream, uint64_t n, const uint32_t* in, uint16_t* out);
 cudaError_t launch_mlp_grad_finalize(cudaStream_t stream, uint32_t n, float* dw_accum, __half* gradients);
 
 // General (unfused) training path: loss + dL/d(output) from fp16 prediction rows [batch][stride]; data_pdf ([batch][n_out], divides the
@@ -63,7 +72,8 @@ cudaError_t launch_dp_barrier(cudaStream_t stream, const DpPeers& peers, uint32_
 // ranks of grads[r][i] (multimem.ld_reduce in the switch, or peer loads), evaluated once by the slice's owner; the updated fp16
 // weight is published into every rank's params (multimem.st, or peer stores); the reduced gradient is left in the local gradient
 // buffer. State arrays (fp32 master, moments, steps) are local and indexed by the global parameter index.
+template <typename Step>
 cudaError_t launch_adam_step_dp(cudaStream_t stream, const AdamParams& a, const DpPeers& peers, uint64_t first, uint64_t count, uint32_t n_matrix_weights, uint64_t n_params,
-                                float loss_scale, float* weights_full_precision, float* first_moments, float* second_moments, uint32_t* param_steps);
+                                float loss_scale, float* weights_full_precision, float* first_moments, float* second_moments, Step* param_steps);
 
 }  // namespace tcnnb

@@ -142,6 +142,12 @@ struct Model {
 	__half* params_fp16 = nullptr;
 	__half* grads_fp16 = nullptr;
 	DeviceBuffer<float> first_moments, second_moments;
+	// Per-parameter Adam step counters: 16-bit (saturating at 65535) when adam_u16_steps_exact() proves the updates identical, else
+	// 32-bit. With 16-bit counters, param_steps is the uint32 view that tcnnb_optimizer_state hands out, widened on demand; while it is
+	// live it is authoritative and is narrowed back before the next consumer (steps32 / sync_steps).
+	bool steps16 = false;
+	bool steps_mirror_live = false;
+	DeviceBuffer<uint16_t> param_steps16;
 	DeviceBuffer<uint32_t> param_steps;
 	DeviceBuffer<float> dw_accum;   // fp32 MLP weight-gradient accumulator
 	DeviceBuffer<float> scalars;    // [0] = loss sum
@@ -256,6 +262,49 @@ static const char* fused_kernel_unsupported(const EncodingPlan& plan, const MlpC
 	if (fused_ws_smem_bytes(mlp.n_hidden_layers, plan.width, true) > 227 * 1024) return "shared-memory footprint of this depth / encoding width";
 	if (grid && grid->interpolation == INTERP_NEAREST) return "Nearest interpolation";
 	return nullptr;
+}
+
+// The uint32 step counters: the state itself, or (16-bit counters) the mirror, widened on `stream` unless it is already live.
+static uint32_t* steps32(Model& m, cudaStream_t stream) {
+	if (m.steps16 && !m.steps_mirror_live) {
+		m.param_steps.resize(m.n_params);
+		TCNNB_CUDA_CHECK(launch_widen_steps(stream, m.n_params, m.param_steps16.ptr, m.param_steps.ptr));
+		m.steps_mirror_live = true;
+	}
+	return m.param_steps.ptr;
+}
+
+// Makes the 16-bit counters current again after a caller wrote through the uint32 mirror (saturating: exact, see
+// adam_u16_steps_exact).
+static void sync_steps(Model& m, cudaStream_t stream) {
+	if (m.steps16 && m.steps_mirror_live) {
+		TCNNB_CUDA_CHECK(launch_narrow_steps(stream, m.n_params, m.param_steps.ptr, m.param_steps16.ptr));
+		m.steps_mirror_live = false;
+	}
+}
+
+// Selects the counter layout, carrying the current counts over. Synchronous.
+static void set_step_counter_width(Model& m, bool use16) {
+	if (use16 == m.steps16 && (use16 ? m.param_steps16.n : m.param_steps.n) == m.n_params) return;
+	TCNNB_CUDA_CHECK(cudaDeviceSynchronize());
+	if (use16) {
+		const bool carry = m.param_steps.n == m.n_params;
+		m.param_steps16.resize(m.n_params);
+		if (carry) TCNNB_CUDA_CHECK(launch_narrow_steps(nullptr, m.n_params, m.param_steps.ptr, m.param_steps16.ptr));
+		else m.param_steps16.zero();
+		m.param_steps.release();
+	} else {
+		m.param_steps.resize(m.n_params);
+		if (m.param_steps16.n == m.n_params) {
+			if (!m.steps_mirror_live) TCNNB_CUDA_CHECK(launch_widen_steps(nullptr, m.n_params, m.param_steps16.ptr, m.param_steps.ptr));
+		} else {
+			m.param_steps.zero();
+		}
+		m.param_steps16.release();
+	}
+	m.steps16 = use16;
+	m.steps_mirror_live = false;
+	TCNNB_CUDA_CHECK(cudaDeviceSynchronize());
 }
 
 static void build_model(Model& m, uint32_t n_in, uint32_t n_out, const json::Value& cfg, uint32_t seed, bool module_only = false) {
@@ -392,8 +441,9 @@ static void build_model(Model& m, uint32_t n_in, uint32_t n_out, const json::Val
 		m.first_moments.zero();
 		m.second_moments.resize(m.n_params);
 		m.second_moments.zero();
-		m.param_steps.resize(m.n_params);
-		m.param_steps.zero();
+		bool exact = false;
+		TCNNB_CUDA_CHECK(adam_u16_steps_exact(m.adam, &exact));
+		set_step_counter_width(m, exact);
 	}
 	m.dw_accum.resize(mlp.n_params);
 	m.dw_accum.zero();
@@ -473,6 +523,7 @@ static AdamParams next_adam_params(Model& m) {
 static void optimizer_step(Model& m, cudaStream_t stream, uint32_t n_ranges = 0, const uint64_t* begins = nullptr, const uint64_t* counts = nullptr) {
 	if (m.module_only) throw std::runtime_error("this handle was created with tcnnb_module_create: it has no optimizer.");
 	m.wait_pending(stream);
+	sync_steps(m, stream);
 	const AdamParams a = next_adam_params(m);
 	const uint64_t whole_begin = 0, whole_count = m.n_params;
 	if (n_ranges == 0) {
@@ -489,9 +540,14 @@ static void optimizer_step(Model& m, cudaStream_t stream, uint32_t n_ranges = 0,
 		const uint32_t n_matrix = b < m.mlp.n_params ? (uint32_t)(m.mlp.n_params - b) : 0u;  // matrix weights inside this range
 		covers_mlp |= b == 0 && n_matrix > 0;
 		if (n_matrix > 0 && b != 0) throw std::runtime_error("optimizer_step: the network weights must be covered from parameter 0.");
-		TCNNB_CUDA_CHECK(launch_adam_step(stream, a, (uint32_t)c, n_matrix, m.loss_scale, m.params_fp32 + b, m.params_fp16 + b, m.grads_fp16 + b,
-		                                  (m.mlp_grads_in_accum && n_matrix > 0) ? m.dw_accum.ptr : nullptr, m.first_moments.ptr + b, m.second_moments.ptr + b,
-		                                  m.param_steps.ptr + b));
+		float* const dw = (m.mlp_grads_in_accum && n_matrix > 0) ? m.dw_accum.ptr : nullptr;
+		if (m.steps16) {
+			TCNNB_CUDA_CHECK(launch_adam_step(stream, a, (uint32_t)c, n_matrix, m.loss_scale, m.params_fp32 + b, m.params_fp16 + b, m.grads_fp16 + b, dw, m.first_moments.ptr + b,
+			                                  m.second_moments.ptr + b, m.param_steps16.ptr + b));
+		} else {
+			TCNNB_CUDA_CHECK(launch_adam_step(stream, a, (uint32_t)c, n_matrix, m.loss_scale, m.params_fp32 + b, m.params_fp16 + b, m.grads_fp16 + b, dw, m.first_moments.ptr + b,
+			                                  m.second_moments.ptr + b, m.param_steps.ptr + b));
+		}
 		++g_kernel_launches;
 	}
 	if (covers_mlp) m.mlp_grads_in_accum = false;
@@ -685,9 +741,15 @@ static void dp_training_step(Model& m, cudaStream_t stream, uint32_t shard_batch
 		// weights into every replica (multimem.st / peer stores) -> [barrier: all slices have landed everywhere; the gradient
 		// vectors may be zeroed again]. No NCCL call on the step.
 		TCNNB_CUDA_CHECK(launch_dp_barrier(stream, d.peers, ++d.epoch));
+		sync_steps(m, stream);
 		const AdamParams a = next_adam_params(m);
-		TCNNB_CUDA_CHECK(launch_adam_step_dp(stream, a, d.peers, lo, chunk, (uint32_t)m.mlp.n_params, m.n_params, m.loss_scale, m.params_fp32, m.first_moments.ptr, m.second_moments.ptr,
-		                                     m.param_steps.ptr));
+		if (m.steps16) {
+			TCNNB_CUDA_CHECK(launch_adam_step_dp(stream, a, d.peers, lo, chunk, (uint32_t)m.mlp.n_params, m.n_params, m.loss_scale, m.params_fp32, m.first_moments.ptr,
+			                                     m.second_moments.ptr, m.param_steps16.ptr));
+		} else {
+			TCNNB_CUDA_CHECK(launch_adam_step_dp(stream, a, d.peers, lo, chunk, (uint32_t)m.mlp.n_params, m.n_params, m.loss_scale, m.params_fp32, m.first_moments.ptr,
+			                                     m.second_moments.ptr, m.param_steps.ptr));
+		}
 		TCNNB_CUDA_CHECK(launch_dp_barrier(stream, d.peers, ++d.epoch));
 		g_kernel_launches += 3;
 		d.masters_synced = false;
@@ -1148,9 +1210,12 @@ int tcnnb_optimizer_state(tcnnb_model* m, float** first_moments_dev, float** sec
 		throw std::runtime_error("optimizer state is sharded over the data-parallel ranks: each rank holds the moments of its own slice only");
 	}
 	TCNNB_CUDA_CHECK(cudaDeviceSynchronize());
+	if (param_steps_dev) {
+		*param_steps_dev = steps32(mm, nullptr);
+		TCNNB_CUDA_CHECK(cudaDeviceSynchronize());
+	}
 	if (first_moments_dev) *first_moments_dev = mm.first_moments.ptr;
 	if (second_moments_dev) *second_moments_dev = mm.second_moments.ptr;
-	if (param_steps_dev) *param_steps_dev = mm.param_steps.ptr;
 	if (current_step) *current_step = mm.adam_step_count;
 	if (base_learning_rate) *base_learning_rate = mm.adam.learning_rate;
 	TCNNB_API_END
@@ -1158,6 +1223,10 @@ int tcnnb_optimizer_state(tcnnb_model* m, float** first_moments_dev, float** sec
 
 int tcnnb_set_optimizer_progress(tcnnb_model* m, uint32_t current_step, float base_learning_rate) {
 	TCNNB_API_BEGIN
+	if (!m->impl.module_only) {  // the caller may have just written the counters through tcnnb_optimizer_state's pointer
+		sync_steps(m->impl, nullptr);
+		TCNNB_CUDA_CHECK(cudaDeviceSynchronize());
+	}
 	m->impl.adam_step_count = current_step;
 	m->impl.adam.learning_rate = base_learning_rate;
 	TCNNB_API_END
@@ -1287,7 +1356,7 @@ int tcnnb_serialize(tcnnb_model* m, void* dst_host, uint64_t size, int with_opti
 		p += n * 4;
 		TCNNB_CUDA_CHECK(cudaMemcpy(p, mm.second_moments.ptr, n * 4, cudaMemcpyDeviceToHost));
 		p += n * 4;
-		TCNNB_CUDA_CHECK(cudaMemcpy(p, mm.param_steps.ptr, n * 4, cudaMemcpyDeviceToHost));
+		TCNNB_CUDA_CHECK(cudaMemcpy(p, steps32(mm, nullptr), n * 4, cudaMemcpyDeviceToHost));  // uint32 on disk whatever the counters' width
 	}
 	TCNNB_API_END
 }
@@ -1315,7 +1384,10 @@ int tcnnb_deserialize(tcnnb_model* m, const void* src_host, uint64_t size) {
 		p += n * 4;
 		TCNNB_CUDA_CHECK(cudaMemcpy(mm.second_moments.ptr, p, n * 4, cudaMemcpyHostToDevice));
 		p += n * 4;
+		if (mm.steps16) mm.param_steps.resize(n);
 		TCNNB_CUDA_CHECK(cudaMemcpy(mm.param_steps.ptr, p, n * 4, cudaMemcpyHostToDevice));
+		mm.steps_mirror_live = mm.steps16;
+		sync_steps(mm, nullptr);
 		mm.adam_step_count = st;
 	}
 	TCNNB_CUDA_CHECK(cudaDeviceSynchronize());
@@ -1523,6 +1595,12 @@ int tcnnb_debug_set(tcnnb_model* m, const char* key, int value) {
 	TCNNB_API_BEGIN
 	const std::string k = key ? key : "";
 	if (k == "binning") m->impl.binning = value != 0;
+	else if (k == "adam_steps32") {  // 32-bit step counters although 16-bit ones give the same updates (tests compare the two layouts)
+		if (m->impl.module_only) throw std::runtime_error("tcnnb_debug_set(adam_steps32): this handle has no optimizer.");
+		bool exact = false;
+		if (!value) TCNNB_CUDA_CHECK(adam_u16_steps_exact(m->impl.adam, &exact));
+		set_step_counter_width(m->impl, exact);
+	}
 	else if (k == "general") {
 		// the stand-alone kernels have their own limits (e.g. dL/d(encoded) wider than the layers): only switch when they cover the configuration
 		if (value && !m->impl.general) {
