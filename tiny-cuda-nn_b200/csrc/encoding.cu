@@ -3,7 +3,8 @@
 // Mirrors tcnn::cpp::create_encoding (cpp_api.h:124, src/cpp_api.cu:165-174: a DifferentiableObject<__half> around
 // create_encoding<__half>(n_input_dims, json, alignment 0)), i.e. what the PyTorch extension's tcnn.Encoding binds
 // (bindings.cpp:284-343), for "Grid" / "HashGrid" / "TiledGrid" / "DenseGrid", "Identity", "Frequency", "TriangleWave", "OneBlob",
-// "SphericalHarmonics" and "Composite" of those (src/encoding.cu:60-120):
+// "SphericalHarmonics", "Empty", "Composite" of those with the Concatenation / Sum / Product reductions and "NRC" / "OneBlobFrequency"
+// (src/encoding.cu:60-120):
 //   forward / inference   fp32 inputs [n][n_input_dims] -> fp16 features [n][n_output_dims]
 //   backward              dL_dparams (fp16, OVERWRITTEN; grids only) and / or dL_dinput fp32 from dL_doutput
 //   backward_backward_input  second-order derivatives of a single grid (grid.h:910-1042, grid_bwd_bwd.cu); every other
@@ -114,11 +115,11 @@ int tcnnb_encoding_backward(tcnnb_encoding* e, tcnnb_stream stream, uint32_t n_e
 	check_ptr(input_dev, "input", 4);
 	check_ptr(dL_doutput_dev, "dL_doutput", enc.max_align);
 	if (dL_dparams_dev && plan.n_params) check_ptr(dL_dparams_dev, "dL_dparams", enc.max_align);
-	if (dL_dinput_dev && !plan.grids.empty()) check_ptr(params_dev, "params", enc.max_align);
-	cudaStream_t s = (cudaStream_t)stream;
-	const __half* dy = (const __half*)dL_doutput_dev;
-	if (dL_dparams_dev) plan_param_gradients(plan, s, n_elements, input_dev, dy, plan.width, (__half*)dL_dparams_dev, enc.max_level);  // GradientMode::Overwrite (src/cpp_api.cu:115)
-	if (dL_dinput_dev) plan_input_gradient(plan, s, n_elements, input_dev, (const __half*)params_dev, dy, plan.width, dL_dinput_dev, enc.max_level);
+	// a Product recomputes the nested outputs from (input, params): nothing of an earlier forward call is read
+	if ((dL_dinput_dev || (dL_dparams_dev && plan.reduction == REDUCE_PRODUCT)) && !plan.grids.empty()) check_ptr(params_dev, "params", enc.max_align);
+	// GradientMode::Overwrite (src/cpp_api.cu:115)
+	plan_backward(plan, (cudaStream_t)stream, n_elements, input_dev, (const __half*)params_dev, (const __half*)dL_doutput_dev, plan.width, (__half*)dL_dparams_dev, dL_dinput_dev,
+	              enc.max_level);
 	TCNNB_API_END
 }
 

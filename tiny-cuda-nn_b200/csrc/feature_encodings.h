@@ -6,7 +6,7 @@
 
 namespace tcnnb {
 
-enum FeatureType : uint32_t { FEAT_IDENTITY = 0, FEAT_FREQUENCY = 1, FEAT_TRIANGLE_WAVE = 2, FEAT_ONEBLOB = 3, FEAT_SPHERICAL_HARMONICS = 4, FEAT_GRID = 5 };
+enum FeatureType : uint32_t { FEAT_IDENTITY = 0, FEAT_FREQUENCY = 1, FEAT_TRIANGLE_WAVE = 2, FEAT_ONEBLOB = 3, FEAT_SPHERICAL_HARMONICS = 4, FEAT_GRID = 5, FEAT_EMPTY = 6 };
 
 struct FeatureSegment {
 	uint32_t type;
@@ -14,6 +14,7 @@ struct FeatureSegment {
 	uint32_t out_begin;          // first output column
 	uint32_t n_out;              // features (without padding)
 	uint32_t n_pad;              // padding columns, all ONE (the grid pads with zeros): behind the features, IN FRONT for SphericalHarmonics
+	                             // (FEAT_EMPTY: no features, only its padding; the kernels write nothing else for it)
 	uint32_t param;              // n_frequencies / log2(n_bins) / degree
 	float scale, offset;         // Identity
 };

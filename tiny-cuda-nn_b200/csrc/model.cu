@@ -608,8 +608,8 @@ static void general_backward_pass(Model& m, cudaStream_t stream, uint32_t batch,
 	run_mlp_backward(mlp, m.g_mlp, m.n_sms, stream, batch, params, m.g_enc.ptr, m.g_mlp.hidden.ptr, out_rows, dL_doutput, ext_dL_doutput != nullptr,
 	                 need_denc ? m.g_denc.ptr : nullptr, want_param_grads ? m.dw_accum.ptr : nullptr);
 	if (want_param_grads) m.mlp_grads_in_accum = true;
-	if (grid_params) plan_param_gradients(m.plan, stream, batch, x, m.g_denc.ptr, mlp.in_width, grads + mlp.n_params, 1.0f);
-	if (dL_dinput) plan_input_gradient(m.plan, stream, batch, x, params + mlp.n_params, m.g_denc.ptr, mlp.in_width, dL_dinput, 1.0f);
+	// (a Product reads the nested outputs general_forward just left in the plan's scratch)
+	plan_backward(m.plan, stream, batch, x, params + mlp.n_params, m.g_denc.ptr, mlp.in_width, grid_params ? grads + mlp.n_params : nullptr, dL_dinput, 1.0f, true);
 	m.last_stream = stream;
 	m.prof_mark(stream);
 }

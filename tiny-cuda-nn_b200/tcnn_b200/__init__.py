@@ -5,6 +5,8 @@ This mirrors, in Python, the names a user of the reference touches on this path:
 `.trainer.loss()`, `.network.inference(...)` (config.h:46-63, trainer.h:254-378, object.h:214).
 It is plumbing for tests and bench.py: torch is used only for device memory and streams. There is no CPU
 fallback -- if the CUDA library is missing or the device is not an sm_90 (H100-class) GPU, construction raises.
+Encodings: the grids, Identity, Frequency, TriangleWave, OneBlob, SphericalHarmonics, Empty, Composite with the Concatenation / Sum /
+Product reductions and dims_to_encode_begin, and the NRC / OneBlobFrequency shorthand, in every tier.
 """
 import ctypes
 import json

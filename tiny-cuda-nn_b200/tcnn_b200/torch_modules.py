@@ -131,7 +131,8 @@ class NetworkWithInputEncoding(_TcnnModule):
 
 
 class Encoding(_TcnnModule):
-    """tinycudann.Encoding (modules.py:312-330): grids, Identity, Frequency, TriangleWave, OneBlob, SphericalHarmonics, Composite; fp16 features."""
+    """tinycudann.Encoding (modules.py:312-330): grids, Identity, Frequency, TriangleWave, OneBlob, SphericalHarmonics, Empty, Composite
+    (Concatenation / Sum / Product, dims_to_encode_begin) and the NRC shorthand; fp16 features."""
 
     def __init__(self, n_input_dims, encoding_config, seed=1337):
         self.encoding_config = encoding_config
