@@ -169,7 +169,7 @@ int tcnnb_encoding_backward_backward_input(tcnnb_encoding* e, tcnnb_stream strea
  * tcnn::cpp::create_network (cpp_api.h:122; src/cpp_api.cu:160-162 = the same network behind the Identity encoding).
  * `network_json` carries the reference's keys ("otype", "n_neurons", "n_hidden_layers", "activation", "output_activation"); both
  * "FullyFusedMLP" and "CutlassMLP"/"MLP" run on the wgmma kernel of csrc/mlp_fused.cu (widths 16/32/64/128, any depth >= 1,
- * padded outputs up to n_neurons). Parameters are CALLER-owned fp16 device arrays (16-byte aligned) in the reference's layout
+ * padded outputs up to 1024, also wider than n_neurons). Parameters are CALLER-owned fp16 device arrays (16-byte aligned) in the reference's layout
  * (fully_fused_mlp.cu:635-672): W_0 [n_neurons][input_width], (n_hidden_layers - 1) x [n_neurons][n_neurons],
  * W_out [padded_output_width][n_neurons], row-major; input_width = n_input_dims rounded up to 16.
  * Hidden activations: FullyFusedMLP's set (everything but Sine / SiLU); "CutlassMLP"/"MLP" also take Sine and SiLU, whose derivative

@@ -5,7 +5,8 @@ untouched:
     python scripts/compare_sass.py old/mlp_fused.o new/mlp_fused.o
 
 Instruction text is compared with addresses and column padding removed. A kernel template that gained a trailing `bool` parameter
-(`mlp_forward_kernel<W, GENERIC_ACT, BWD, PRE>`, `fused_ws_kernel<D, F, TRAIN, GENERIC_ACT, PDF>`) is matched to its old name when the new parameter is false. Exit code 1 if any old
+(`mlp_forward_kernel<W, GENERIC_ACT, BWD, PRE, WIDE>`, `fused_ws_kernel<D, F, TRAIN, GENERIC_ACT, PDF>`, `mlp_wgrad_kernel<W, WIDE>`) is matched to its old name
+when the new parameter is false. Exit code 1 if any old
 kernel is missing or differs.
 
 Build both objects from the same source path (e.g. stash the change, build, unstash, build): kernels in an anonymous namespace
@@ -29,7 +30,7 @@ def functions(obj):
 
 
 def old_name(name):
-    return re.sub(r"(I(?:Lj\d+E)+Lb\dELb\d)ELb0(EE)", r"\1\2", name)
+    return re.sub(r"(I(?:L[jb]\d+E)+)Lb0E(E)", r"\1\2", name)
 
 
 def main():

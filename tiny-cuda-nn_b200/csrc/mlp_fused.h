@@ -10,7 +10,7 @@ struct MlpChainParams {
 	// row-major fp16, contiguous in this order
 	uint32_t width;              // 16 / 32 / 64 / 128 / 256
 	uint32_t in_width;           // multiple of 16, <= max(width, 64) ... see mlp_forward_supported()
-	uint32_t out_width;          // PADDED output width: multiple of 16, <= width rounded up to 64
+	uint32_t out_width;          // PADDED output width: multiple of 16, <= MLP_MAX_OUTPUT_WIDTH (wider than `width`: the WIDE kernels)
 	uint32_t n_hidden_layers;    // >= 1
 	uint32_t activation;         // hidden activation (Activation enum)
 	uint32_t output_activation;
@@ -44,6 +44,10 @@ struct MlpForwardParams : MlpChainParams {
 	// Kept out of MlpChainParams so that the parameter block of the other activations' kernels keeps its layout.
 	__half* hidden_pre_out;
 };
+
+// Widest padded network output the stand-alone kernels run. An output wider than n_neurons is computed in chunks of n_neurons rows of
+// the output matrix (the WIDE kernels).
+constexpr uint32_t MLP_MAX_OUTPUT_WIDTH = 1024;
 
 // Maximum number of weight matrices that stay resident in shared memory for a width (more layers stream through a ring).
 uint32_t mlp_forward_resident_layers(uint32_t width);

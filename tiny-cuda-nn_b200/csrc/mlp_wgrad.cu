@@ -45,7 +45,10 @@ struct WgradKernelParams {
 
 }  // namespace
 
-template <uint32_t W>
+// WIDE = true: dL/d(output) is wider than an accumulator (out_width > NMAX, the widest fan-in). The output matrix then takes
+// n_ob = ceil(out_width / NMAX) passes over the CTA's tiles, pass c accumulating dW_out rows NMAX c .. NMAX c + NMAX - 1 from
+// dL/d(output) columns of the same range; every pass fetches h_{NH-1} again.
+template <uint32_t W, bool WIDE>
 __global__ void __launch_bounds__(WgradCfg<W>::THREADS, 1)
 mlp_wgrad_kernel(const WgradKernelParams kp, const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_h, const __grid_constant__ CUtensorMap map_g,
                  const __grid_constant__ CUtensorMap map_go) {
@@ -57,7 +60,9 @@ mlp_wgrad_kernel(const WgradKernelParams kp, const __grid_constant__ CUtensorMap
 	const uint32_t lane = tid & 31u;
 	const uint32_t NH = p.n_hidden_layers;
 	const uint32_t in_w = p.in_width, out_w = p.out_width;
-	const uint32_t n_matrices = NH + 1;
+	constexpr uint32_t NMAX = C::KB * 64;  // widest fan-in
+	const uint32_t n_ob = WIDE ? (out_w + NMAX - 1) / NMAX : 1u;  // passes of the output matrix
+	const uint32_t n_matrices = NH + n_ob;
 
 	const uint32_t smem_base = smem_u32(smem_raw);
 	if (smem_base & 1023u) __trap();
@@ -85,7 +90,8 @@ mlp_wgrad_kernel(const WgradKernelParams kp, const __grid_constant__ CUtensorMap
 	const uint32_t tile_begin = (uint32_t)((uint64_t)blockIdx.x * n_tiles / gridDim.x), tile_end = (uint32_t)((uint64_t)(blockIdx.x + 1) * n_tiles / gridDim.x);
 	const uint32_t n_my = tile_end - tile_begin;
 	const uint32_t n_items = n_my * n_matrices;  // (matrix, tile) pairs, tile fastest
-	auto b_cols_of = [&](uint32_t mi) { return mi == 0 ? in_w : (mi == NH ? out_w : W); };
+	auto b_cols_of = [&](uint32_t mi) { return WIDE ? (mi == 0 ? in_w : (mi < NH ? W : min(NMAX, out_w - (mi - NH) * NMAX))) : (mi == 0 ? in_w : (mi == NH ? out_w : W)); };
+	auto ob_of = [&](uint32_t mi) { return WIDE && mi > NH ? mi - NH : 0u; };  // pass of the output matrix
 
 	if (warp == C::WGS * 4) {
 		// =================================================================================== TMA producer
@@ -108,7 +114,7 @@ mlp_wgrad_kernel(const WgradKernelParams kp, const __grid_constant__ CUtensorMap
 				for (uint32_t b = 0; b < b_boxes; ++b) {
 					if (mi == 0) tma_load_2d(b_dst + b * TILE_BYTES, &map_x, full, (int32_t)(b * 64), row);
 					else if (mi < NH) tma_load_2d(b_dst + b * TILE_BYTES, &map_h, full, (int32_t)(b * 64), (int32_t)((mi - 1) * p.batch_size) + row);
-					else tma_load_2d(b_dst + b * TILE_BYTES, &map_go, full, (int32_t)(b * 64), row);
+					else tma_load_2d(b_dst + b * TILE_BYTES, &map_go, full, (int32_t)(b * 64 + ob_of(mi) * NMAX), row);
 				}
 			}
 		}
@@ -116,7 +122,6 @@ mlp_wgrad_kernel(const WgradKernelParams kp, const __grid_constant__ CUtensorMap
 		// =================================================================================== consumer warpgroup h: accumulator rows 64 h ..
 		const uint32_t h = warp / 4, wq = warp & 3u;
 		const uint32_t fq = lane >> 2, ft = lane & 3u;
-		constexpr uint32_t NMAX = C::KB * 64;  // widest fan-in
 		float d[NMAX / 2];
 		for (uint32_t it = 0; it < n_items; ++it) {
 			const uint32_t mi = it / n_my;
@@ -142,7 +147,7 @@ mlp_wgrad_kernel(const WgradKernelParams kp, const __grid_constant__ CUtensorMap
 			if (lane == 0) mbar_arrive_plain(bar_free + 8 * stage);
 			if (!last_tile) continue;
 			// ---- flush: partial sums -> global fp32. d[4 i + q]: row m = 64 h + 16 wq + lane / 4 (+ 8 for q >= 2), column 8 i + 2 (lane % 4) + (q & 1)
-			float* base = p.dw_accum + (mi == 0 ? 0 : (size_t)W * in_w + (size_t)(mi - 1) * W * W);
+			float* base = p.dw_accum + (mi == 0 ? 0 : (size_t)W * in_w + (size_t)((WIDE ? min(mi, NH) : mi) - 1) * W * W) + (size_t)ob_of(mi) * NMAX * W;
 #pragma unroll
 			for (uint32_t i = 0; i < NMAX / 8; ++i) {
 				const uint32_t n = 8 * i + 2 * ft;
@@ -182,9 +187,9 @@ struct Wgrad256 {
 	static constexpr uint32_t THREADS = WGS * 128 + 32;
 };
 
-__global__ void __launch_bounds__(Wgrad256::THREADS, 1)
-mlp_wgrad256_kernel(const WgradKernelParams kp, const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_h, const __grid_constant__ CUtensorMap map_g,
-                    const __grid_constant__ CUtensorMap map_go) {
+// WIDE = true (out_width > 256): the output matrix takes n_ob = ceil(out_width / 256) passes, as in mlp_wgrad_kernel.
+template <bool WIDE>
+__device__ __forceinline__ void wgrad256_body(const WgradKernelParams& kp, const CUtensorMap& map_x, const CUtensorMap& map_h, const CUtensorMap& map_g, const CUtensorMap& map_go) {
 	using C = Wgrad256;
 	constexpr uint32_t W = C::W;
 	const MlpWgradParams& p = kp.p;
@@ -194,7 +199,8 @@ mlp_wgrad256_kernel(const WgradKernelParams kp, const __grid_constant__ CUtensor
 	const uint32_t lane = tid & 31u;
 	const uint32_t NH = p.n_hidden_layers;
 	const uint32_t in_w = p.in_width, out_w = p.out_width;
-	const uint32_t n_matrices = NH + 1;
+	const uint32_t n_ob = WIDE ? (out_w + W - 1) / W : 1u;
+	const uint32_t n_matrices = NH + n_ob;
 
 	const uint32_t smem_base = smem_u32(smem_raw);
 	if (smem_base & 1023u) __trap();
@@ -222,7 +228,8 @@ mlp_wgrad256_kernel(const WgradKernelParams kp, const __grid_constant__ CUtensor
 	const uint32_t tile_begin = (uint32_t)((uint64_t)pair * n_tiles / n_pairs), tile_end = (uint32_t)((uint64_t)(pair + 1) * n_tiles / n_pairs);
 	const uint32_t n_my = tile_end - tile_begin;
 	const uint32_t n_items = n_my * n_matrices;
-	auto b_cols_of = [&](uint32_t mi) { return mi == 0 ? in_w : (mi == NH ? out_w : W); };
+	auto b_cols_of = [&](uint32_t mi) { return WIDE ? (mi == 0 ? in_w : (mi < NH ? W : min(W, out_w - (mi - NH) * W))) : (mi == 0 ? in_w : (mi == NH ? out_w : W)); };
+	auto ob_of = [&](uint32_t mi) { return WIDE && mi > NH ? mi - NH : 0u; };
 
 	if (warp == C::WGS * 4) {
 		// =================================================================================== TMA producer
@@ -244,7 +251,7 @@ mlp_wgrad256_kernel(const WgradKernelParams kp, const __grid_constant__ CUtensor
 				for (uint32_t b = 0; b < b_boxes; ++b) {
 					if (mi == 0) tma_load_2d(b_dst + b * TILE_BYTES, &map_x, full, (int32_t)(b * 64), row);
 					else if (mi < NH) tma_load_2d(b_dst + b * TILE_BYTES, &map_h, full, (int32_t)(b * 64), (int32_t)((mi - 1) * p.batch_size) + row);
-					else tma_load_2d(b_dst + b * TILE_BYTES, &map_go, full, (int32_t)(b * 64), row);
+					else tma_load_2d(b_dst + b * TILE_BYTES, &map_go, full, (int32_t)(b * 64 + ob_of(mi) * W), row);
 				}
 			}
 		}
@@ -279,7 +286,7 @@ mlp_wgrad256_kernel(const WgradKernelParams kp, const __grid_constant__ CUtensor
 			if (lane == 0) mbar_arrive_plain(bar_free + 8 * stage);
 			if (!last_tile) continue;
 			// ---- flush, as mlp_wgrad_kernel: d[4 i + q] = row m, column 8 i + 2 (lane % 4) + (q & 1)
-			float* base = p.dw_accum + (mi == 0 ? 0 : (size_t)W * in_w + (size_t)(mi - 1) * W * W);
+			float* base = p.dw_accum + (mi == 0 ? 0 : (size_t)W * in_w + (size_t)((WIDE ? min(mi, NH) : mi) - 1) * W * W) + (size_t)ob_of(mi) * W * W;
 #pragma unroll
 			for (uint32_t i = 0; i < W / 8; ++i) {
 				const uint32_t n = 8 * i + 2 * ft;
@@ -302,6 +309,18 @@ mlp_wgrad256_kernel(const WgradKernelParams kp, const __grid_constant__ CUtensor
 	pdl_launch_dependents();
 }
 
+__global__ void __launch_bounds__(Wgrad256::THREADS, 1)
+mlp_wgrad256_kernel(const WgradKernelParams kp, const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_h, const __grid_constant__ CUtensorMap map_g,
+                    const __grid_constant__ CUtensorMap map_go) {
+	wgrad256_body<false>(kp, map_x, map_h, map_g, map_go);
+}
+
+__global__ void __launch_bounds__(Wgrad256::THREADS, 1)
+mlp_wgrad256_wide_kernel(const WgradKernelParams kp, const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_h, const __grid_constant__ CUtensorMap map_g,
+                         const __grid_constant__ CUtensorMap map_go) {
+	wgrad256_body<true>(kp, map_x, map_h, map_g, map_go);
+}
+
 namespace {
 
 cudaError_t launch_wgrad256(const MlpWgradParams& p, uint32_t n_sms, cudaStream_t stream, uint32_t* n_launches) {
@@ -313,18 +332,19 @@ cudaError_t launch_wgrad256(const MlpWgradParams& p, uint32_t n_sms, cudaStream_
 	if (!make_fp16_matrix_map(&mg, p.grad_hidden, (uint64_t)NH * B, C::W, TILE_M)) return cudaErrorInvalidValue;
 	if (!make_fp16_matrix_map(&mgo, p.grad_output, B, p.out_width, TILE_M)) return cudaErrorInvalidValue;
 	const size_t smem = (size_t)C::STAGES * C::STAGE_BYTES + 8 * 2 * C::STAGES;
-	cudaError_t err = cudaFuncSetAttribute(mlp_wgrad256_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+	auto kernel = p.out_width > C::W ? mlp_wgrad256_wide_kernel : mlp_wgrad256_kernel;
+	cudaError_t err = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
 	if (err != cudaSuccess) return err;
 	const uint32_t n_tiles = B / TILE_M, n_pairs = n_tiles < n_sms / 2 ? n_tiles : n_sms / 2;
 	WgradKernelParams kp{};
 	kp.p = p;
-	err = launch_pdl(mlp_wgrad256_kernel, 2 * n_pairs, C::THREADS, smem, stream, kp, mx, mh, mg, mgo);
+	err = launch_pdl(kernel, 2 * n_pairs, C::THREADS, smem, stream, kp, mx, mh, mg, mgo);
 	if (err != cudaSuccess) return err;
 	if (n_launches) ++*n_launches;
 	return cudaSuccess;
 }
 
-template <uint32_t W>
+template <uint32_t W, bool WIDE>
 cudaError_t launch_wgrad_width(const MlpWgradParams& p, uint32_t n_sms, cudaStream_t stream, uint32_t* n_launches) {
 	using C = WgradCfg<W>;
 	const uint32_t NH = p.n_hidden_layers, B = p.batch_size;
@@ -333,7 +353,7 @@ cudaError_t launch_wgrad_width(const MlpWgradParams& p, uint32_t n_sms, cudaStre
 	if (!make_fp16_matrix_map(&mh, p.hidden, (uint64_t)NH * B, W, TILE_M)) return cudaErrorInvalidValue;
 	if (!make_fp16_matrix_map(&mg, p.grad_hidden, (uint64_t)NH * B, W, TILE_M)) return cudaErrorInvalidValue;
 	if (!make_fp16_matrix_map(&mgo, p.grad_output, B, p.out_width, TILE_M)) return cudaErrorInvalidValue;
-	auto kernel = mlp_wgrad_kernel<W>;
+	auto kernel = mlp_wgrad_kernel<W, WIDE>;
 	const size_t smem = (size_t)C::STAGES * C::STAGE_BYTES + 8 * 2 * C::STAGES;
 	cudaError_t err = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
 	if (err != cudaSuccess) return err;
@@ -344,6 +364,12 @@ cudaError_t launch_wgrad_width(const MlpWgradParams& p, uint32_t n_sms, cudaStre
 	if (err != cudaSuccess) return err;
 	if (n_launches) ++*n_launches;
 	return cudaSuccess;
+}
+
+// dL/d(output) wider than an accumulator (64 columns below 128 neurons, 128 at 128) takes the WIDE kernel
+template <uint32_t W>
+cudaError_t launch_wgrad_width(const MlpWgradParams& p, uint32_t n_sms, cudaStream_t stream, uint32_t* n_launches) {
+	return p.out_width > WgradCfg<W>::KB * 64 ? launch_wgrad_width<W, true>(p, n_sms, stream, n_launches) : launch_wgrad_width<W, false>(p, n_sms, stream, n_launches);
 }
 
 }  // namespace
@@ -357,7 +383,8 @@ bool mlp_wgrad_supported(const MlpWgradParams& p, const char** why) {
 	if (p.n_hidden_layers < 1) return fail("FullyFusedMLP requires at least 1 hidden layer (3 layers in total).");
 	const uint32_t max_in = 64 * ((p.width + 63) / 64);
 	if (p.in_width == 0 || p.in_width % 16 != 0 || p.in_width > max_in) return fail("tcnn_b200: network input width must be a multiple of 16 and at most 64 (128 / 256 for 128 / 256 neurons)");
-	if (p.out_width == 0 || p.out_width % 16 != 0 || p.out_width > max_in) return fail("tcnn_b200: padded network output width must be a multiple of 16 and at most n_neurons");
+	if (p.out_width == 0 || p.out_width % 16 != 0) return fail("tcnn_b200: padded network output width must be a multiple of 16 and at most n_neurons");
+	if (p.out_width > MLP_MAX_OUTPUT_WIDTH) return fail("tcnn_b200: padded network output width must be at most 1024");
 	if (p.batch_size == 0 || p.batch_size % TILE_M != 0) return fail("batch size must be a non-zero multiple of 256");
 	if ((uint64_t)p.n_hidden_layers * p.batch_size >= (1ull << 31)) return fail("tcnn_b200: n_hidden_layers * batch_size must stay below 2^31 rows");
 	return true;
