@@ -83,7 +83,15 @@ int tcnnb_set_params(tcnnb_model* m, const void* params_half, uint64_t n, int de
  * the fp32 first / second moments and the uint32 per-parameter step counters ([n_params] each; valid for the model's lifetime),
  * the optimizer's step counter and base learning rate. Synchronises the device. */
 int tcnnb_optimizer_state(tcnnb_model* m, float** first_moments_dev, float** second_moments_dev, uint32_t** param_steps_dev, uint32_t* current_step, float* base_learning_rate);
+/* Restores the optimizer's step counter and base learning rate (the undecayed one under ExponentialDecay). ExponentialDecay's
+ * learning-rate factor is recomputed from the step counter, exactly as an uninterrupted run reaches it; tcnnb_deserialize does the same. */
 int tcnnb_set_optimizer_progress(tcnnb_model* m, uint32_t current_step, float base_learning_rate);
+/* ExponentialDecay's current learning-rate factor (optimizers/exponential_decay.h `learning_rate_factor`; 1 without the wrapper): the
+ * next step runs at base_learning_rate * factor, times decay_base when that step is a decay boundary. The setter overrides the factor
+ * that tcnnb_set_optimizer_progress recomputed, for snapshots that store their own (the reference's ExponentialDecay schema); it fails
+ * when the optimizer has no ExponentialDecay wrapper. */
+float tcnnb_learning_rate_factor(const tcnnb_model* m);
+int tcnnb_set_learning_rate_factor(tcnnb_model* m, float factor);
 
 /* ---- trainer->training_step(stream, input, target, ..., run_optimizer) (trainer.h:254-357) ----
  * input_dev [batch][n_in] fp32, target_dev [batch][n_out] fp32, both device pointers.

@@ -18,6 +18,7 @@
 #include <nlohmann/json.hpp>
 #endif
 
+#include <cctype>
 #include <memory>
 #include <string>
 #include <vector>
@@ -172,7 +173,9 @@ public:
 
 	/* trainer.h:442-482 + optimizers/adam.h:303-325: the reference's snapshot schema (nlohmann binary values; instant-ngp stores it as
 	 * msgpack): {"n_params", "params_type": "__half", "params_binary", "optimizer": {"current_step", "base_learning_rate",
-	 * "first_moments_binary", "second_moments_binary", "param_steps_binary"}}. Snapshots written by tiny-cuda-nn load here and vice versa. */
+	 * "first_moments_binary", "second_moments_binary", "param_steps_binary"}}. Under ExponentialDecay the Adam state is nested as in
+	 * optimizers/exponential_decay.h:136-148: "optimizer": {"nested": {Adam's keys, with base_learning_rate the DECAYED rate},
+	 * "learning_rate": the undecayed base rate, "learning_rate_factor"}. Snapshots written by tiny-cuda-nn load here and vice versa. */
 	json serialize(bool serialize_optimizer = false) {
 		const size_t n = n_params();
 		auto blob = [](const void* dev, size_t bytes) {
@@ -190,13 +193,19 @@ public:
 			float *m1 = nullptr, *m2 = nullptr, lr = 0;
 			uint32_t *steps = nullptr, cur = 0;
 			TCNNB_CHECK_THROW(tcnnb_optimizer_state(m_handle->m, &m1, &m2, &steps, &cur, &lr));
+			const bool decay = exponential_decay();
+			const float factor = tcnnb_learning_rate_factor(m_handle->m);
 			json opt;
 			opt["current_step"] = cur;
-			opt["base_learning_rate"] = lr;
+			opt["base_learning_rate"] = decay ? lr * factor : lr;  /* the nested Adam runs at the decayed rate (exponential_decay.h:69) */
 			opt["first_moments_binary"] = blob(m1, n * sizeof(float));
 			opt["second_moments_binary"] = blob(m2, n * sizeof(float));
 			opt["param_steps_binary"] = blob(steps, n * sizeof(uint32_t));
-			data["optimizer"] = opt;
+			if (decay) {
+				data["optimizer"] = {{"nested", opt}, {"learning_rate", lr}, {"learning_rate_factor", factor}};
+			} else {
+				data["optimizer"] = opt;
+			}
 		}
 		return data;
 	}
@@ -224,7 +233,9 @@ public:
 			throw std::runtime_error{"Trainer: snapshot parameters must be of type float of __half"};
 		}
 		if (data.contains("optimizer")) {
-			const json& opt = data["optimizer"];
+			/* ExponentialDecay's schema nests the Adam state; a flat one (the wrapper's factor then follows from the step count) loads too */
+			const bool nested = exponential_decay() && data["optimizer"].contains("nested");
+			const json& opt = nested ? data["optimizer"]["nested"] : data["optimizer"];
 			float *m1 = nullptr, *m2 = nullptr;
 			uint32_t* steps = nullptr;
 			TCNNB_CHECK_THROW(tcnnb_optimizer_state(m_handle->m, &m1, &m2, &steps, nullptr, nullptr));
@@ -239,7 +250,11 @@ public:
 			} else {
 				CUDA_CHECK_THROW(cudaMemset(steps, 0, n * sizeof(uint32_t)));
 			}
-			TCNNB_CHECK_THROW(tcnnb_set_optimizer_progress(m_handle->m, opt.at("current_step").get<uint32_t>(), opt.at("base_learning_rate").get<float>()));
+			const float base_lr = nested ? data["optimizer"].at("learning_rate").get<float>() : opt.at("base_learning_rate").get<float>();
+			TCNNB_CHECK_THROW(tcnnb_set_optimizer_progress(m_handle->m, opt.at("current_step").get<uint32_t>(), base_lr));
+			if (nested && data["optimizer"].contains("learning_rate_factor")) {
+				TCNNB_CHECK_THROW(tcnnb_set_learning_rate_factor(m_handle->m, data["optimizer"]["learning_rate_factor"].get<float>()));
+			}
 		}
 		CUDA_CHECK_THROW(cudaDeviceSynchronize());
 	}
@@ -252,6 +267,13 @@ public:
 	tcnnb_model* handle() const { return m_handle->m; }
 
 private:
+	/* whether the optimizer is Adam inside ExponentialDecay (src/optimizer.cu compares names case-insensitively) */
+	bool exponential_decay() const {
+		std::string name = m_optimizer->hyperparams().value("otype", std::string{"Adam"});
+		for (char& c : name) c = (char)std::tolower((unsigned char)c);
+		return name == "exponentialdecay";
+	}
+
 	std::shared_ptr<NetworkWithInputEncoding<COMPUTE_T>> m_model;
 	std::shared_ptr<Optimizer<PARAMS_T>> m_optimizer;
 	std::shared_ptr<Loss<COMPUTE_T>> m_loss;

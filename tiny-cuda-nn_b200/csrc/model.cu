@@ -499,6 +499,27 @@ static FusedStepParams make_params(const Model& m, uint32_t batch, uint32_t loss
 	return p;
 }
 
+// ExponentialDecay's learning-rate factor after `n_steps` uninterrupted steps: the schedule of next_adam_params replayed with the
+// same float multiplications, so that a trainer whose step count is restored continues bit-identically. Each decay boundary is
+// visited once; the loop stops early once a multiplication no longer changes the factor (0, 1 or a saturated value).
+static float lr_decay_factor_after(const Model& m, uint32_t n_steps) {
+	float factor = 1.0f;
+	if (!m.lr_decay.enabled || n_steps == 0) return factor;
+	const uint64_t last = std::min<uint64_t>((uint64_t)n_steps - 1, m.lr_decay.end);
+	for (uint64_t step = m.lr_decay.start; step <= last; step += m.lr_decay.interval) {
+		const float next = factor * m.lr_decay.base;
+		if (next == factor) break;
+		factor = next;
+	}
+	return factor;
+}
+
+// Sets the optimizer's step count from outside (a snapshot, tcnnb_set_optimizer_progress); the decay factor follows it.
+static void restore_adam_step_count(Model& m, uint32_t n_steps) {
+	m.adam_step_count = n_steps;
+	m.lr_decay.factor = lr_decay_factor_after(m, n_steps);
+}
+
 // Hyper-parameters of the next optimizer step (advances the step counter; AdaBound bounds per adam.h:161-168).
 static AdamParams next_adam_params(Model& m) {
 	if (m.lr_decay.enabled) {  // exponential_decay.h:60-70, evaluated with the step count BEFORE this step
@@ -758,7 +779,7 @@ static void dp_training_step(Model& m, cudaStream_t stream, uint32_t shard_batch
 	TCNNB_NCCL_CHECK(n.ReduceScatter(m.grads_fp16, m.grads_fp16 + lo, chunk, ncclHalf, ncclSum, d.comm_grads, stream));
 	const uint64_t begin = lo, count = lo < m.n_params ? std::min<uint64_t>(chunk, m.n_params - lo) : 0;
 	if (count) optimizer_step(m, stream, 1, &begin, &count);
-	else ++m.adam_step_count;
+	else (void)next_adam_params(m);  // a rank with no parameters in its slice still advances the step count and the decay schedule
 	TCNNB_CUDA_CHECK(cudaEventRecord(d.ev_updated, stream));
 	TCNNB_CUDA_CHECK(cudaStreamWaitEvent(d.gather_stream, d.ev_updated, 0));
 	TCNNB_NCCL_CHECK(n.AllGather(m.params_fp16 + lo, m.params_fp16, chunk, ncclHalf, d.comm_params, d.gather_stream));
@@ -1227,8 +1248,19 @@ int tcnnb_set_optimizer_progress(tcnnb_model* m, uint32_t current_step, float ba
 		sync_steps(m->impl, nullptr);
 		TCNNB_CUDA_CHECK(cudaDeviceSynchronize());
 	}
-	m->impl.adam_step_count = current_step;
+	restore_adam_step_count(m->impl, current_step);
 	m->impl.adam.learning_rate = base_learning_rate;
+	TCNNB_API_END
+}
+
+// ExponentialDecay's learning-rate factor (exponential_decay.h:136-148 `learning_rate_factor`; 1 without the wrapper). Setting the
+// step count recomputes it from the schedule; a snapshot that stores its own factor restores it here afterwards.
+float tcnnb_learning_rate_factor(const tcnnb_model* m) { return m->impl.lr_decay.factor; }
+
+int tcnnb_set_learning_rate_factor(tcnnb_model* m, float factor) {
+	TCNNB_API_BEGIN
+	if (!m->impl.lr_decay.enabled) throw std::runtime_error("set_learning_rate_factor: the optimizer has no ExponentialDecay wrapper.");
+	m->impl.lr_decay.factor = factor;
 	TCNNB_API_END
 }
 
@@ -1388,7 +1420,7 @@ int tcnnb_deserialize(tcnnb_model* m, const void* src_host, uint64_t size) {
 		TCNNB_CUDA_CHECK(cudaMemcpy(mm.param_steps.ptr, p, n * 4, cudaMemcpyHostToDevice));
 		mm.steps_mirror_live = mm.steps16;
 		sync_steps(mm, nullptr);
-		mm.adam_step_count = st;
+		restore_adam_step_count(mm, st);
 	}
 	TCNNB_CUDA_CHECK(cudaDeviceSynchronize());
 	TCNNB_API_END

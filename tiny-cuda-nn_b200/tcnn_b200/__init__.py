@@ -62,6 +62,8 @@ ABI = [
     ("tcnnb_set_params", _int, [_vp, _vp, _u64, _int]),
     ("tcnnb_optimizer_state", _int, [_vp, ctypes.POINTER(_vp), ctypes.POINTER(_vp), ctypes.POINTER(_vp), ctypes.POINTER(_u32), _f32p]),
     ("tcnnb_set_optimizer_progress", _int, [_vp, _u32, ctypes.c_float]),
+    ("tcnnb_learning_rate_factor", ctypes.c_float, [_vp]),
+    ("tcnnb_set_learning_rate_factor", _int, [_vp, ctypes.c_float]),
     ("tcnnb_training_step", _int, [_vp, _vp, _u32, _vp, _vp, _int]),
     ("tcnnb_training_step_ex", _int, [_vp, _vp, _u32, _vp, _vp, _vp, _int, _vp, _int, _int, _vp]),
     ("tcnnb_training_step_shard", _int, [_vp, _vp, _u32, _u32, _vp, _vp, _int]),
