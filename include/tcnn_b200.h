@@ -226,6 +226,10 @@ int tcnnb_network_module_inference(tcnnb_network* n, tcnnb_stream stream, uint32
  * [n_ctas][5 roles][64 events][8 fields] at clocks_dev (null = off): role = consumer warpgroup (4 unused), event = round * n_steps +
  * step, fields 0..3 = waiting for the weights / weights ready / product complete / epilogue done. Not part of the drop-in surface. */
 int tcnnb_network_debug_clocks(tcnnb_network* n, void* clocks_dev);
+/* Tests only: the following backward passes write g_l = dL/d(pre-activation of hidden layer l), the rows the weight-gradient kernel
+ * reads, to grad_hidden_dev (fp16 [n_hidden_layers][n_elements][n_neurons], 16-byte aligned; null = the network's own scratch), with
+ * or without dL/dparams. Not part of the drop-in surface. */
+int tcnnb_network_debug_grad_hidden(tcnnb_network* n, void* grad_hidden_dev);
 
 /* ---- data parallelism, natively over NCCL (no counterpart in the single-GPU reference; SURVEY.md section 8e) -------------
  * One process per GPU. Rendezvous is the host framework's job (torch.distributed in tcnn_b200/dp.py): rank 0 draws two NCCL

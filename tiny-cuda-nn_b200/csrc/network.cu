@@ -88,11 +88,13 @@ void run_mlp_backward(const MlpConfig& c, MlpScratch& s, int n_sms, cudaStream_t
 	a.output = output;
 	a.dL_doutput = dL_doutput;
 	a.dL_dinput = dL_dinput;
-	if (dw_accum) {
+	if (s.grad_hidden_tap) {
+		a.grad_hidden = s.grad_hidden_tap;
+	} else if (dw_accum) {
 		grow(s.grad_hidden, (size_t)c.n_hidden_layers * batch * c.width);
 		a.grad_hidden = s.grad_hidden.ptr;
-		a.dw_accum = dw_accum;
 	}
+	a.dw_accum = dw_accum;
 	if (a.output_activation != ACT_NONE) {
 		grow(s.grad_output, (size_t)batch * c.padded_out_width);
 		a.grad_output = s.grad_output.ptr;
@@ -191,6 +193,13 @@ uint32_t tcnnb_network_n_forward_activations(const tcnnb_network* n) { return n_
 int tcnnb_network_debug_clocks(tcnnb_network* n, void* clocks_dev) {
 	TCNNB_API_BEGIN
 	n->impl.dbg_clock = (long long*)clocks_dev;
+	TCNNB_API_END
+}
+
+int tcnnb_network_debug_grad_hidden(tcnnb_network* n, void* grad_hidden_dev) {
+	TCNNB_API_BEGIN
+	if ((uintptr_t)grad_hidden_dev % 16 != 0) throw std::runtime_error("network: grad_hidden must be 16-byte aligned.");
+	n->impl.scratch.grad_hidden_tap = (__half*)grad_hidden_dev;
 	TCNNB_API_END
 }
 

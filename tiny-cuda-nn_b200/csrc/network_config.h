@@ -102,6 +102,9 @@ struct MlpScratch {
 	DeviceBuffer<__half> hidden;       // activations kept by a forward pass (hidden_rows)
 	DeviceBuffer<__half> grad_hidden;  // g_l = dL/d(pre-activation of hidden layer l), for the weight gradients
 	DeviceBuffer<__half> grad_output;  // dL/d(output) through the output activation
+	// tests only (tcnnb_network_debug_grad_hidden): when set, the backward pass writes g_l here instead of `grad_hidden`, with or
+	// without weight gradients -- [n_hidden_layers][batch][width] fp16, owned by the caller
+	__half* grad_hidden_tap = nullptr;
 	__half* hidden_rows(const MlpConfig& c, uint32_t batch);
 };
 

@@ -100,6 +100,7 @@ ABI = [
     ("tcnnb_network_module_backward", _int, [_vp, _vp, _u32, _vp, _vp, _vp, _vp, _vp]),
     ("tcnnb_network_inference", _int, [_vp, _vp, _u32, _vp, _vp, _vp]),
     ("tcnnb_network_debug_clocks", _int, [_vp, _vp]),
+    ("tcnnb_network_debug_grad_hidden", _int, [_vp, _vp]),
     ("tcnnb_network_module_inference", _int, [_vp, _vp, _u32, _vp, _vp, _vp]),
     ("tcnnb_dp_unique_id", _int, [_vp, ctypes.c_uint64]),
     ("tcnnb_dp_init", _int, [_vp, _vp, _vp, ctypes.c_int, ctypes.c_int, ctypes.c_int]),
@@ -663,6 +664,16 @@ class Network:
     def bwd_bwd_input(self, *args, **kwargs):
         """Second-order derivatives are built for the grid encodings alone (Encoding.bwd_bwd_input), as in the reference."""
         raise TcnnError("Network does not support double backward.")
+
+    def set_debug_grad_hidden(self, grad_hidden=None):
+        """Tests only: later backward calls write g_l (dL/d pre-activation of every hidden layer) into `grad_hidden`, fp16
+        [n_hidden_layers][n][width] on the device; None hands the rows back to the network's own scratch."""
+        import torch
+
+        if grad_hidden is not None:
+            assert grad_hidden.dtype == torch.float16 and grad_hidden.is_cuda and grad_hidden.is_contiguous()
+        self._grad_hidden = grad_hidden  # kept alive while the network writes to it
+        _check(load().tcnnb_network_debug_grad_hidden(self._h, grad_hidden.data_ptr() if grad_hidden is not None else None))
 
     def inference(self, x32, params16, stream=None):
         """fp32 [n][n_input_dims] through the Identity encoding -> fp32 [n][n_output_dims]."""
