@@ -149,13 +149,19 @@ struct Model {
 	bool steps_mirror_live = false;
 	DeviceBuffer<uint16_t> param_steps16;
 	DeviceBuffer<uint32_t> param_steps;
+	// Calls f with the live counters (uint16_t* or uint32_t*): the Adam kernels are instantiated for both widths.
+	template <typename F>
+	void with_step_counters(F&& f) {
+		if (steps16) f(param_steps16.ptr);
+		else f(param_steps.ptr);
+	}
 	DeviceBuffer<float> dw_accum;   // fp32 MLP weight-gradient accumulator
 	DeviceBuffer<float> scalars;    // [0] = loss sum
 	DeviceBuffer<long long> dbg_clock;  // TCNNB_CLOCKS=<file> in ablation builds: phase stamps of the last ws launch
 	FusedStepParams fused{};                // the fused kernel's per-model arguments (configurations it runs); make_params adds the per-call ones
-	DeviceBuffer<__half> denc_scratch;      // module tier: dL/d(encoded) rows [n][64] handed from the fused kernel to the input-gradient kernel
-	DeviceBuffer<__half> grads_scratch;     // module tier: gradient array when the caller wants dL/d(input) only; trainer: GradientMode::Ignore / Accumulate
-	DeviceBuffer<float> dw_scratch;         // trainer, GradientMode::Ignore: network weight-gradient sums nobody reads
+	DeviceBuffer<__half> denc_scratch;      // fused path, dL/d(input): dL/d(encoded) rows [n][64] handed from the fused kernel to the input-gradient kernel
+	DeviceBuffer<__half> grads_scratch;     // GradientMode::Ignore (fused path): table gradients nobody reads; Accumulate (general path): this call's table gradients
+	DeviceBuffer<float> dw_scratch;         // GradientMode::Ignore (fused path): network weight-gradient sums nobody reads
 	bool mlp_grads_in_accum = false;
 	// General (unfused) path: configurations the fused kernel does not cover -- 128 neurons, n_features_per_level in {1, 4, 8}, 4-D
 	// inputs, Nearest interpolation, wider encodings / outputs -- run as encoding kernel -> stand-alone MLP kernels -> encoding backward
@@ -206,7 +212,7 @@ struct Model {
 	// optional per-kernel timing (bench.py roofline): events around the fused kernel and the Adam kernel of every step
 	uint32_t ablate = 0;  // profiling experiments only (TCNNB_ABLATE env var)
 	bool profiling = false;
-	std::vector<cudaEvent_t> prof_events;  // quadruples: step start, after binning, after fused kernel, after Adam
+	std::vector<cudaEvent_t> prof_events;  // quadruples: step start, after binning, after the backward pass, after Adam
 
 	~Model() {
 		if (pinned) cudaFreeHost(pinned);
@@ -479,13 +485,13 @@ static void build_model(Model& m, uint32_t n_in, uint32_t n_out, const json::Val
 	}
 }
 
-static FusedStepParams make_params(const Model& m, uint32_t batch, uint32_t loss_batch, const float* x, const float* y) {
+static FusedStepParams make_params(const Model& m, uint32_t batch, uint32_t loss_batch, const float* x, const float* y, const __half* params) {
 	FusedStepParams p = m.fused;
 	p.batch_size = batch;
 	p.loss_batch_size = loss_batch;
 	p.positions = x;
 	p.targets = y;
-	p.params = m.params_fp16;
+	p.params = params;
 	p.grads = m.grads_fp16;
 	p.dw_accum = m.dw_accum.ptr;
 	p.loss_sum = m.scalars.ptr;
@@ -562,13 +568,10 @@ static void optimizer_step(Model& m, cudaStream_t stream, uint32_t n_ranges = 0,
 		covers_mlp |= b == 0 && n_matrix > 0;
 		if (n_matrix > 0 && b != 0) throw std::runtime_error("optimizer_step: the network weights must be covered from parameter 0.");
 		float* const dw = (m.mlp_grads_in_accum && n_matrix > 0) ? m.dw_accum.ptr : nullptr;
-		if (m.steps16) {
+		m.with_step_counters([&](auto* steps) {
 			TCNNB_CUDA_CHECK(launch_adam_step(stream, a, (uint32_t)c, n_matrix, m.loss_scale, m.params_fp32 + b, m.params_fp16 + b, m.grads_fp16 + b, dw, m.first_moments.ptr + b,
-			                                  m.second_moments.ptr + b, m.param_steps16.ptr + b));
-		} else {
-			TCNNB_CUDA_CHECK(launch_adam_step(stream, a, (uint32_t)c, n_matrix, m.loss_scale, m.params_fp32 + b, m.params_fp16 + b, m.grads_fp16 + b, dw, m.first_moments.ptr + b,
-			                                  m.second_moments.ptr + b, m.param_steps.ptr + b));
-		}
+			                                  m.second_moments.ptr + b, steps + b));
+		});
 		++g_kernel_launches;
 	}
 	if (covers_mlp) m.mlp_grads_in_accum = false;
@@ -594,104 +597,131 @@ static void general_forward(Model& m, cudaStream_t stream, uint32_t batch, const
 	m.last_stream = stream;
 }
 
-// Forward + loss (or the caller's dL/d(output)) + backward on the general path. Gradients land where the fused kernel leaves them:
-// fp32 network weight-gradient sums in dw_accum, fp16 table gradients in grads + n_mlp_params (overwritten). `dL_dinput` (fp32
-// [batch][n_in]) and `data_pdf` optional; `keep_mlp_accum`: add onto the fp32 sums a previous step left (GradientMode::Accumulate).
-static void general_backward_pass(Model& m, cudaStream_t stream, uint32_t batch, uint32_t loss_batch, const float* x, const float* y, const __half* params, __half* grads,
-                                  const __half* ext_dL_doutput, float* dL_dinput, bool want_param_grads, const float* data_pdf = nullptr, bool keep_mlp_accum = false) {
-	const MlpConfig& mlp = m.mlp;
-	const bool grid_params = m.plan.n_params != 0 && want_param_grads;
-	if (!ext_dL_doutput) TCNNB_CUDA_CHECK(cudaMemsetAsync(m.scalars.ptr, 0, sizeof(float), stream));
-	if (m.mlp_grads_in_accum && !keep_mlp_accum) {
-		TCNNB_CUDA_CHECK(cudaMemsetAsync(m.dw_accum.ptr, 0, sizeof(float) * mlp.n_params, stream));
+__global__ void half_to_float_kernel(uint64_t n, const __half* __restrict__ in, float* __restrict__ out) {
+	const uint64_t i = threadIdx.x + (uint64_t)blockIdx.x * blockDim.x;
+	if (i < n) out[i] = (float)in[i];
+}
+
+__global__ void half_accumulate_kernel(uint64_t n, const __half* __restrict__ in, __half* __restrict__ inout) {
+	const uint64_t i = threadIdx.x + (uint64_t)blockIdx.x * blockDim.x;
+	if (i < n) inout[i] = __hadd(inout[i], in[i]);
+}
+
+// tcnn::GradientMode (object.h:116-120)
+enum GradientMode : int { GRADIENT_IGNORE = 0, GRADIENT_OVERWRITE = 1, GRADIENT_ACCUMULATE = 2 };
+
+// One backward call of the trainer or module tier: Trainer::training_step with all of its arguments (trainer.h:254-357) or
+// Module::backward (cpp_api.cu:104-125).
+struct BackwardCall {
+	uint32_t batch = 0, loss_batch = 0;  // loss_batch: what the loss is normalised over (the global batch of a data-parallel shard)
+	const float* x = nullptr;
+	const float* y = nullptr;             // targets (unused with dL_doutput)
+	const float* data_pdf = nullptr;      // optional [batch][n_out]: the loss divides by it
+	const __half* params = nullptr;       // the trainer's working or Ema weights, or the module caller's
+	const __half* dL_doutput = nullptr;   // optional fp16 [batch][padded_out_width], already x loss scale: replaces the loss
+	GradientMode mode = GRADIENT_OVERWRITE;
+	__half* grads = nullptr;              // [n_params]: the trainer's gradient buffer or the module caller's dL_dparams
+	float* dL_dinput = nullptr;           // optional fp32 [batch][n_in], overwritten
+	bool finalize = false;                // round the fp32 network sums into `grads` (the module tier hands out fp16 gradients)
+	bool run_optimizer = false;
+	cudaEvent_t targets_ready = nullptr;  // optional: the first kernel waits for it; gradient zeroing and binning only need `x`
+};
+
+// fp32 network weight-gradient sums -> fp16 entries of `grads` (what the reference's gradient buffer holds); re-arms the accumulator
+static void finalize_mlp_grads(Model& m, cudaStream_t stream, __half* grads) {
+	if (m.mlp_grads_in_accum) {
+		TCNNB_CUDA_CHECK(launch_mlp_grad_finalize(stream, m.mlp.n_params, m.dw_accum.ptr, grads));
+		++g_kernel_launches;
 		m.mlp_grads_in_accum = false;
 	}
-	m.prof_mark(stream);
-	m.prof_mark(stream);  // (no binning pass on this path)
-	m.wait_pending(stream);
-	grow(m.g_out, (size_t)batch * mlp.padded_out_width);
+}
+
+// The general path's backward pass: forward with the activations kept, the loss (or the caller's dL/d(output)), the network backward
+// adding into `dw` and the encoding backward overwriting `table_grads` (either may be null) and dL_dinput.
+static void general_backward(Model& m, cudaStream_t stream, const BackwardCall& c, float* dw, __half* table_grads) {
+	const MlpConfig& mlp = m.mlp;
+	grow(m.g_out, (size_t)c.batch * mlp.padded_out_width);
 	__half* const out_rows = (m.taps.output && mlp.padded_out_width == 16) ? (__half*)m.taps.output : m.g_out.ptr;  // (the test tap is 16 columns wide)
-	general_forward(m, stream, batch, x, params, out_rows, nullptr, true);
+	general_forward(m, stream, c.batch, c.x, c.params, out_rows, nullptr, true);
 
 	// Module::backward: the caller's dL/d(output) still has to pass the output activation (fully_fused_mlp.cu:755-762). Trainer: the
 	// loss kernel writes loss gradient x loss_scale, through the output activation, in one kernel.
-	const __half* dL_doutput = ext_dL_doutput;
-	if (!ext_dL_doutput) {
-		grow(m.g_dy, (size_t)batch * mlp.padded_out_width);
+	const __half* dL_doutput = c.dL_doutput;
+	if (!dL_doutput) {
+		grow(m.g_dy, (size_t)c.batch * mlp.padded_out_width);
 		__half* const dy_rows = (m.taps.dL_doutput && mlp.padded_out_width == 16) ? (__half*)m.taps.dL_doutput : m.g_dy.ptr;
-		TCNNB_CUDA_CHECK(launch_loss(stream, m.loss_type, mlp.output_activation, batch, m.n_out, mlp.padded_out_width, m.loss_scale, loss_batch * m.n_out, out_rows, y, data_pdf,
-		                             dy_rows, m.taps.loss_values, m.scalars.ptr));
+		TCNNB_CUDA_CHECK(launch_loss(stream, m.loss_type, mlp.output_activation, c.batch, m.n_out, mlp.padded_out_width, m.loss_scale, c.loss_batch * m.n_out, out_rows, c.y,
+		                             c.data_pdf, dy_rows, m.taps.loss_values, m.scalars.ptr));
 		++g_kernel_launches;
 		dL_doutput = dy_rows;
 	}
-	const bool need_denc = grid_params || dL_dinput;
-	if (need_denc) grow(m.g_denc, (size_t)batch * mlp.in_width);
-	run_mlp_backward(mlp, m.g_mlp, m.n_sms, stream, batch, params, m.g_enc.ptr, m.g_mlp.hidden.ptr, out_rows, dL_doutput, ext_dL_doutput != nullptr,
-	                 need_denc ? m.g_denc.ptr : nullptr, want_param_grads ? m.dw_accum.ptr : nullptr);
-	if (want_param_grads) m.mlp_grads_in_accum = true;
+	const bool need_denc = table_grads || c.dL_dinput;
+	if (need_denc) grow(m.g_denc, (size_t)c.batch * mlp.in_width);
+	run_mlp_backward(mlp, m.g_mlp, m.n_sms, stream, c.batch, c.params, m.g_enc.ptr, m.g_mlp.hidden.ptr, out_rows, dL_doutput, c.dL_doutput != nullptr,
+	                 need_denc ? m.g_denc.ptr : nullptr, dw);
 	// (a Product reads the nested outputs general_forward just left in the plan's scratch)
-	plan_backward(m.plan, stream, batch, x, params + mlp.n_params, m.g_denc.ptr, mlp.in_width, grid_params ? grads + mlp.n_params : nullptr, dL_dinput, 1.0f, true);
-	m.last_stream = stream;
-	m.prof_mark(stream);
+	plan_backward(m.plan, stream, c.batch, c.x, c.params + mlp.n_params, m.g_denc.ptr, mlp.in_width, table_grads, c.dL_dinput, 1.0f, true);
 }
 
-// `targets_ready`: optional event the fused kernel (the first consumer of `y`) waits for; everything before it in the step --
-// gradient zeroing, the binning pass -- only needs `x` and runs while the targets are still in flight.
-// Arrays of a fused step other than the trainer's own: the module tier's caller-owned ones (cpp_api.h:76-104) and the optional arguments
-// of Trainer::training_step (tcnnb_training_step_ex).
-struct ModuleIO {
-	const __half* params = nullptr;
-	__half* grads = nullptr;
-	const __half* dL_doutput = nullptr;  // optional: replaces the loss (targets unused)
-	__half* dL_dencoded = nullptr;  // optional [n][64] fp16: the network's input gradient rows, for the input-position gradient
-	const float* data_pdf = nullptr;  // optional [n][n_out]: the loss divides by it
-	float* dw_accum = nullptr;        // optional: fp32 network weight-gradient sums other than the model's (GradientMode::Ignore)
-	bool accumulate = false;          // add onto `grads` and the fp32 sums instead of overwriting them (GradientMode::Accumulate / Ignore)
-};
-
-static void training_step(Model& m, cudaStream_t stream, uint32_t batch, uint32_t loss_batch, const float* x, const float* y, bool run_optimizer, cudaEvent_t targets_ready = nullptr,
-                          const ModuleIO* io = nullptr) {
-	check_batch(batch);
-	if (!io && m.module_only) throw std::runtime_error("this handle was created with tcnnb_module_create: use the tcnnb_module_* calls.");
-	if (m.use_general()) {
-		if (io) throw std::runtime_error("internal: the module tier of the general path does not come through here");
-		if (targets_ready) TCNNB_CUDA_CHECK(cudaStreamWaitEvent(stream, targets_ready, 0));
-		general_backward_pass(m, stream, batch, loss_batch, x, y, m.params_fp16, m.grads_fp16, nullptr, nullptr, true);
-		if (run_optimizer) optimizer_step(m, stream);
-		m.prof_mark(stream);
-		return;
+// Runs one backward call on the fused kernel or the general path, then the optimizer when asked. Records one profile quadruple.
+static void backward_step(Model& m, cudaStream_t stream, const BackwardCall& c) {
+	const uint32_t batch = c.batch, n_mlp = m.mlp.n_params;
+	const bool general = m.use_general();
+	const bool overwrite = c.mode == GRADIENT_OVERWRITE;
+	if (c.dL_dinput && !general) {
+		// Nothing checks the fused kernel's dL/d(encoded) rows of an Identity encoding; the general path computes this gradient.
+		if (single_encoding(m.plan, FEAT_IDENTITY)) {
+			throw std::runtime_error("input gradients through an Identity encoding are not built for configurations the fused kernel runs; the general path (e.g. n_neurons > 64) computes them.");
+		}
+		// dL/d(input) (NetworkWithInputEncoding::backward -> GridEncoding::backward_impl, grid.h:896-921): the fused kernel hands out
+		// the network's input gradient rows, the plan's grid kernel contracts them with d(encoded)/d(position).
+		grow(m.denc_scratch, (size_t)batch * 64);
 	}
-	__half* const grads_base = io ? io->grads : m.grads_fp16;
-	float* const dw_accum = io && io->dw_accum ? io->dw_accum : m.dw_accum.ptr;
-	const bool overwrite = !(io && io->accumulate);
-	// GradientMode::Overwrite: zero the grid gradient table (grid.h:865-867) and the loss accumulator -- inside the binning pass
-	// when there is one, else as memsets. Accumulate zeroes the loss accumulator only.
-	__half* const grid_grads = grads_base + m.mlp.n_params;
+
+	// Where the gradients go. Overwrite / Accumulate: the network's into the model's fp32 sums, the table's into `grads`; the general
+	// path overwrites the table gradients it computes, so Accumulate sends them to scratch and adds that onto `grads` afterwards.
+	// Ignore: the fused kernel still scatters, into scratch that is never zeroed and never read (trainer.h:338 hands the reference's a
+	// null gradient buffer); the general path computes no parameter gradients.
+	__half* grads = c.grads;
+	float* dw = m.dw_accum.ptr;
+	if (c.mode == GRADIENT_IGNORE && general) {
+		grads = nullptr;
+		dw = nullptr;
+	} else if (c.mode == GRADIENT_IGNORE || (c.mode == GRADIENT_ACCUMULATE && general)) {
+		m.grads_scratch.resize(m.n_params_padded);
+		grads = m.grads_scratch.ptr;
+		if (!general) {
+			m.dw_scratch.resize(n_mlp);
+			dw = m.dw_scratch.ptr;
+		}
+	}
+	if (c.mode == GRADIENT_ACCUMULATE && !m.mlp_grads_in_accum && n_mlp) {
+		// the network's gradients are the fp16 values in the buffer (tcnnb_param_gradients materialised them): the fp32 sums continue
+		// from there
+		half_to_float_kernel<<<(n_mlp + 255) / 256, 256, 0, stream>>>(n_mlp, c.grads, m.dw_accum.ptr);
+		TCNNB_CUDA_CHECK(cudaGetLastError());
+		++g_kernel_launches;
+		m.mlp_grads_in_accum = true;
+	}
+
+	// Overwrite zeroes the fused kernel's grid gradient table (grid.h:865-867), and the loss accumulator is zeroed -- inside the binning
+	// pass when there is one, else as memsets. (The general path overwrites its table gradients itself; a module handle reports no loss.)
+	__half* const grid_grads = grads ? grads + n_mlp : nullptr;
 	const size_t grid_grad_bytes = sizeof(__half) * m.plan.n_params;
-	const bool bin = m.binning && batch >= 16384 && single_encoding(m.plan, FEAT_GRID);  // spatial order only matters to the table gathers
+	const bool bin = !general && m.binning && batch >= 16384 && single_encoding(m.plan, FEAT_GRID);  // spatial order only matters to the table gathers
 	const bool zero_in_binning = overwrite && bin && (((uintptr_t)grid_grads | grid_grad_bytes) & 15u) == 0;
-	if (!zero_in_binning) {
+	if (general) {
+		if (!m.module_only) TCNNB_CUDA_CHECK(cudaMemsetAsync(m.scalars.ptr, 0, sizeof(float), stream));
+	} else if (!zero_in_binning) {
 		if (overwrite) TCNNB_CUDA_CHECK(cudaMemsetAsync(grid_grads, 0, grid_grad_bytes, stream));
 		TCNNB_CUDA_CHECK(cudaMemsetAsync(m.scalars.ptr, 0, sizeof(float), stream));
 	}
 	if (overwrite && m.mlp_grads_in_accum) {
 		// a previous step left un-consumed weight gradients (run_optimizer == false twice in a row): Overwrite semantics
-		TCNNB_CUDA_CHECK(cudaMemsetAsync(m.dw_accum.ptr, 0, sizeof(float) * m.mlp.n_params, stream));
+		TCNNB_CUDA_CHECK(cudaMemsetAsync(m.dw_accum.ptr, 0, sizeof(float) * n_mlp, stream));
+		m.mlp_grads_in_accum = false;
 	}
-	FusedStepParams p = make_params(m, batch, loss_batch, x, y);
-	if (io) {
-		p.params = io->params;
-		p.grads = io->grads;
-		p.dw_accum = dw_accum;
-		p.data_pdf = io->data_pdf;
-		if (io->dL_dencoded) p.dbg_denc = io->dL_dencoded;
-		if (io->dL_doutput) {
-			p.ext_dy = io->dL_doutput;
-			p.targets = nullptr;
-			p.loss_sum = nullptr;
-			p.loss_values = nullptr;
-		}
-	}
+
 	m.prof_mark(stream);
 	// Process the batch in (y, z)-column order: same sums, far fewer distinct memory sectors on the coarse levels (binning.cu).
 	if (bin) {
@@ -705,33 +735,66 @@ static void training_step(Model& m, cudaStream_t stream, uint32_t batch, uint32_
 				m.bin_hist.zero(stream);
 			}
 		}
-		TCNNB_CUDA_CHECK(launch_binning(stream, m.n_in, batch, x, log2_r, m.bin_keys.ptr, m.bin_hist.ptr, m.bin_perm.ptr, zero_in_binning ? grid_grads : nullptr,
+		TCNNB_CUDA_CHECK(launch_binning(stream, m.n_in, batch, c.x, log2_r, m.bin_keys.ptr, m.bin_hist.ptr, m.bin_perm.ptr, zero_in_binning ? grid_grads : nullptr,
 		                                zero_in_binning ? grid_grad_bytes : 0, zero_in_binning ? (float*)m.scalars.ptr : nullptr));
 		g_kernel_launches += 3;
-		p.perm = m.bin_perm.ptr;
 	}
 	m.prof_mark(stream);
-	if (targets_ready) TCNNB_CUDA_CHECK(cudaStreamWaitEvent(stream, targets_ready, 0));
+	if (c.targets_ready) TCNNB_CUDA_CHECK(cudaStreamWaitEvent(stream, c.targets_ready, 0));
 	m.wait_pending(stream);  // e.g. the all-gather of the previous data-parallel step: binning above did not need the parameters
-	// one persistent 640-thread CTA per SM (fused_ws.cu)
-	TCNNB_CUDA_CHECK(launch_fused_ws(p, m.n_in, true,std::min(batch / TILE_M, (uint32_t)m.n_sms), stream));
-	++g_kernel_launches;
-	m.last_stream = stream;
-	m.prof_mark(stream);
-	if (dw_accum == m.dw_accum.ptr) m.mlp_grads_in_accum = true;
-	if (run_optimizer) {
-		optimizer_step(m, stream);
+	if (general) {
+		general_backward(m, stream, c, dw, m.plan.n_params ? grid_grads : nullptr);
+		if (c.mode == GRADIENT_ACCUMULATE && m.plan.n_params) {
+			half_accumulate_kernel<<<(uint32_t)((m.plan.n_params + 255) / 256), 256, 0, stream>>>(m.plan.n_params, grid_grads, c.grads + n_mlp);
+			TCNNB_CUDA_CHECK(cudaGetLastError());
+			++g_kernel_launches;
+		}
+	} else {
+		FusedStepParams p = make_params(m, batch, c.loss_batch, c.x, c.y, c.params);
+		p.grads = grads;
+		p.dw_accum = dw;
+		p.data_pdf = c.data_pdf;
+		if (bin) p.perm = m.bin_perm.ptr;
+		if (c.dL_dinput) p.dbg_denc = m.denc_scratch.ptr;
+		if (c.dL_doutput) {
+			p.ext_dy = c.dL_doutput;
+			p.targets = nullptr;
+			p.loss_sum = nullptr;
+			p.loss_values = nullptr;
+		}
+		// one persistent 640-thread CTA per SM (fused_ws.cu)
+		TCNNB_CUDA_CHECK(launch_fused_ws(p, m.n_in, true,std::min(batch / TILE_M, (uint32_t)m.n_sms), stream));
+		++g_kernel_launches;
 	}
+	m.last_stream = stream;
+	if (c.mode != GRADIENT_IGNORE) m.mlp_grads_in_accum = true;
+	if (c.finalize) finalize_mlp_grads(m, stream, c.grads);
+	if (c.dL_dinput && !general) plan_input_gradient(m.plan, stream, batch, c.x, c.params + n_mlp, m.denc_scratch.ptr, 64, c.dL_dinput, 1.0f);
+	m.prof_mark(stream);
+	// the optimizer comes last: the input gradient reads the parameters the step used
+	if (c.run_optimizer) optimizer_step(m, stream);
 	m.prof_mark(stream);
 }
 
-// fp32 network weight-gradient sums -> fp16 entries of `grads` (what the reference's gradient buffer holds); re-arms the accumulator
-static void finalize_mlp_grads(Model& m, cudaStream_t stream, __half* grads) {
-	if (m.mlp_grads_in_accum) {
-		TCNNB_CUDA_CHECK(launch_mlp_grad_finalize(stream, m.mlp.n_params, m.dw_accum.ptr, grads));
-		++g_kernel_launches;
-		m.mlp_grads_in_accum = false;
-	}
+static void check_trainer(const Model& m) {
+	if (m.module_only) throw std::runtime_error("this handle was created with tcnnb_module_create: use the tcnnb_module_* calls.");
+}
+
+// The trainer's own step: Overwrite into its gradient buffer (tcnnb_training_step / _shard, the host-buffer pipeline, the data-parallel
+// step).
+static void training_step(Model& m, cudaStream_t stream, uint32_t batch, uint32_t loss_batch, const float* x, const float* y, bool run_optimizer, cudaEvent_t targets_ready = nullptr) {
+	check_batch(batch);
+	check_trainer(m);
+	BackwardCall c;
+	c.batch = batch;
+	c.loss_batch = loss_batch;
+	c.x = x;
+	c.y = y;
+	c.params = m.params_fp16;
+	c.grads = m.grads_fp16;
+	c.run_optimizer = run_optimizer;
+	c.targets_ready = targets_ready;
+	backward_step(m, stream, c);
 }
 
 // One data-parallel step, natively over NCCL (tcnn_b200/dp.py has the same logic over torch.distributed; SURVEY.md section 8e).
@@ -764,13 +827,10 @@ static void dp_training_step(Model& m, cudaStream_t stream, uint32_t shard_batch
 		TCNNB_CUDA_CHECK(launch_dp_barrier(stream, d.peers, ++d.epoch));
 		sync_steps(m, stream);
 		const AdamParams a = next_adam_params(m);
-		if (m.steps16) {
+		m.with_step_counters([&](auto* steps) {
 			TCNNB_CUDA_CHECK(launch_adam_step_dp(stream, a, d.peers, lo, chunk, (uint32_t)m.mlp.n_params, m.n_params, m.loss_scale, m.params_fp32, m.first_moments.ptr,
-			                                     m.second_moments.ptr, m.param_steps16.ptr));
-		} else {
-			TCNNB_CUDA_CHECK(launch_adam_step_dp(stream, a, d.peers, lo, chunk, (uint32_t)m.mlp.n_params, m.n_params, m.loss_scale, m.params_fp32, m.first_moments.ptr,
-			                                     m.second_moments.ptr, m.param_steps.ptr));
-		}
+			                                     m.second_moments.ptr, steps));
+		});
 		TCNNB_CUDA_CHECK(launch_dp_barrier(stream, d.peers, ++d.epoch));
 		g_kernel_launches += 3;
 		d.masters_synced = false;
@@ -795,26 +855,24 @@ static void dp_reduce_loss(Model& m, cudaStream_t stream) {
 	}
 }
 
-static void launch_inference(Model& m, const FusedStepParams& p, uint32_t batch, cudaStream_t stream) {
+// Forward pass with `params`: fp16 rows [batch][padded_output_width] (the module tier, column-major padded x n in the reference's
+// terms, cpp_api.cu:82-83) or fp32 [batch][n_out] (Network::inference, object.h:214-282). Nothing is saved for the backward pass --
+// it recomputes the forward inside the fused kernel (the gather + three MMAs per tile are cheaper than writing and re-reading
+// 2 x 64 x n fp16 activations, which is what the reference's context holds).
+static void forward(Model& m, cudaStream_t stream, uint32_t batch, const float* x, const __half* params, __half* out_fp16, float* out_fp32) {
+	m.wait_pending(stream);
+	if (m.use_general()) {
+		general_forward(m, stream, batch, x, params, out_fp16, out_fp32, false);
+		return;
+	}
+	FusedStepParams p = make_params(m, batch, batch, x, nullptr, params);
+	if (out_fp16) p.out_fp16 = out_fp16;  // (else the output tap, when a test set one)
+	p.out_fp32 = out_fp32;
+	p.loss_sum = nullptr;
 	// the warp-specialised kernel without its backward half (measured 0.0885 ms vs 0.127 ms for the bulk-synchronous kernel it replaced)
 	TCNNB_CUDA_CHECK(launch_fused_ws(p, m.n_in, false,std::min(batch / TILE_M, (uint32_t)m.n_sms), stream));
 	++g_kernel_launches;
 	m.last_stream = stream;
-}
-
-static void inference(Model& m, cudaStream_t stream, uint32_t batch, const float* x, float* out) {
-	check_batch(batch);
-	if (m.module_only) throw std::runtime_error("this handle was created with tcnnb_module_create: use the tcnnb_module_* calls.");
-	m.wait_pending(stream);
-	if (m.use_general()) {
-		general_forward(m, stream, batch, x, m.inference_params(), nullptr, out, false);
-		return;
-	}
-	FusedStepParams p = make_params(m, batch, batch, x, nullptr);
-	p.params = m.inference_params();
-	p.out_fp32 = out;
-	p.loss_sum = nullptr;
-	launch_inference(m, p, batch, stream);
 }
 
 // ---- module tier (tcnn::cpp::Module for NetworkWithInputEncoding, cpp_api.cu:71-158): caller-owned parameters -------------
@@ -823,65 +881,51 @@ static void check_module_ptr(const void* ptr, const char* what) {
 	if ((uintptr_t)ptr % 16 != 0) throw std::runtime_error(std::string("module: ") + what + " must be 16-byte aligned.");
 }
 
-// inference / forward: fp16 [n][padded_output_width] rows (column-major padded x n in the reference's terms, cpp_api.cu:82-83).
-// Nothing is saved for the backward pass -- it recomputes the forward inside the fused kernel (the gather + three MMAs per
-// tile are cheaper than writing and re-reading 2 x 64 x n fp16 activations, which is what the reference's context holds).
-static void module_forward(Model& m, cudaStream_t stream, uint32_t n, const float* x, void* output, const void* params) {
-	check_batch(n);
-	check_module_ptr(params, "params");
-	check_module_ptr(output, "output");
-	if (m.use_general()) {
-		general_forward(m, stream, n, x, (const __half*)params, (__half*)output, nullptr, false);
-		return;
-	}
-	FusedStepParams p = make_params(m, n, n, x, nullptr);
-	p.params = (const __half*)params;
-	p.grads = nullptr;
-	p.out_fp16 = (__half*)output;
-	p.out_fp32 = nullptr;
-	p.loss_sum = nullptr;
-	launch_inference(m, p, n, stream);
-}
-
-// backward: dL_dparams (fp16 [n_params], OVERWRITTEN -- GradientMode::Overwrite, cpp_api.cu:115) from dL_doutput (fp16 [n][padded]).
+// backward: dL_dparams (fp16 [n_params], OVERWRITTEN -- GradientMode::Overwrite, cpp_api.cu:115; Ignore when it is null) from
+// dL_doutput (fp16 [n][padded]).
 static void module_backward(Model& m, cudaStream_t stream, uint32_t n, float* dL_dinput, const void* dL_doutput, void* dL_dparams, const float* x, const void* params) {
-	if (!dL_dparams && !dL_dinput) return;  // nothing to compute (GradientMode::Ignore)
+	if (!dL_dparams && !dL_dinput) return;  // nothing to compute
 	check_module_ptr(params, "params");
 	check_module_ptr(dL_doutput, "dL_doutput");
-	if (m.use_general()) {
-		check_batch(n);
-		if (dL_dparams) check_module_ptr(dL_dparams, "dL_dparams");
-		general_backward_pass(m, stream, n, n, x, nullptr, (const __half*)params, (__half*)dL_dparams, (const __half*)dL_doutput, dL_dinput, dL_dparams != nullptr);
-		finalize_mlp_grads(m, stream, (__half*)dL_dparams);  // (nothing is accumulated without dL_dparams)
-		return;
+	check_batch(n);
+	if (dL_dparams) check_module_ptr(dL_dparams, "dL_dparams");
+	BackwardCall c;
+	c.batch = c.loss_batch = n;
+	c.x = x;
+	c.params = (const __half*)params;
+	c.dL_doutput = (const __half*)dL_doutput;
+	c.mode = dL_dparams ? GRADIENT_OVERWRITE : GRADIENT_IGNORE;
+	c.grads = (__half*)dL_dparams;
+	c.dL_dinput = dL_dinput;
+	c.finalize = dL_dparams != nullptr;
+	backward_step(m, stream, c);
+}
+
+// Trainer::training_step with all of its arguments (trainer.h:254-357): the loss weighted by `data_pdf`, or the caller's `ext_dL_dy`
+// (fp16 [batch][padded_output_width], already x loss scale) in place of the loss; the gradients overwrite, add onto or leave alone the
+// trainer's buffer; `dL_dinput` (fp32 [batch][n_in]) is overwritten.
+static void training_step_ex(Model& m, cudaStream_t stream, uint32_t batch, const float* x, const float* y, const float* data_pdf, bool run_optimizer, float* dL_dinput,
+                             bool use_inference_params, int mode, const __half* ext_dL_dy) {
+	check_trainer(m);
+	if (m.dp) throw std::runtime_error("training_step_ex: data-parallel handles train with tcnnb_dp_training_step.");
+	if (mode != GRADIENT_IGNORE && mode != GRADIENT_OVERWRITE && mode != GRADIENT_ACCUMULATE) {
+		throw std::runtime_error("training_step_ex: param_gradients_mode must be 0 (Ignore), 1 (Overwrite) or 2 (Accumulate).");
 	}
-	// Nothing checks the fused kernel's dL/d(encoded) rows of an Identity encoding; the general path computes this gradient.
-	if (dL_dinput && single_encoding(m.plan, FEAT_IDENTITY)) {
-		throw std::runtime_error("module: input gradients through an Identity encoding are not built for configurations the fused kernel runs; the general path (e.g. n_neurons > 64) computes them.");
-	}
-	ModuleIO io;
-	io.params = (const __half*)params;
-	io.dL_doutput = (const __half*)dL_doutput;
-	if (dL_dparams) {
-		check_module_ptr(dL_dparams, "dL_dparams");
-		io.grads = (__half*)dL_dparams;
-	} else {  // input gradients only: the fused kernel still needs somewhere to scatter
-		m.grads_scratch.resize(m.n_params_padded);
-		io.grads = m.grads_scratch.ptr;
-	}
-	if (dL_dinput) {
-		// dL/d(input) (cpp_api.cu:104-125 -> NetworkWithInputEncoding::backward -> GridEncoding::backward_impl, grid.h:896-921): the fused
-		// kernel hands out the network's input gradient rows, the plan's grid kernel contracts them with d(encoded)/d(position).
-		m.denc_scratch.resize(std::max(m.denc_scratch.n, (size_t)n * 64));
-		io.dL_dencoded = m.denc_scratch.ptr;
-	}
-	if (m.mlp_grads_in_accum) {
-		TCNNB_CUDA_CHECK(cudaMemsetAsync(m.dw_accum.ptr, 0, sizeof(float) * m.mlp.n_params, stream));
-		m.mlp_grads_in_accum = false;
-	}
-	training_step(m, stream, n, n, x, nullptr, false, nullptr, &io);
-	finalize_mlp_grads(m, stream, io.grads);
-	if (dL_dinput) plan_input_gradient(m.plan, stream, n, x, (const __half*)params + m.mlp.n_params, m.denc_scratch.ptr, 64, dL_dinput, 1.0f);
+	if (!ext_dL_dy && !y) throw std::runtime_error("training_step: target is null and no external_dL_dy replaces the loss.");
+	if (!x) throw std::runtime_error("training_step: input is null.");
+	check_batch(batch);
+	BackwardCall c;
+	c.batch = c.loss_batch = batch;
+	c.x = x;
+	c.y = y;
+	c.data_pdf = ext_dL_dy ? nullptr : data_pdf;  // the loss is not evaluated (trainer.h:127-131)
+	c.params = use_inference_params ? m.inference_params() : m.params_fp16;
+	c.dL_doutput = ext_dL_dy;
+	c.mode = (GradientMode)mode;
+	c.grads = m.grads_fp16;
+	c.dL_dinput = dL_dinput;
+	c.run_optimizer = run_optimizer;
+	backward_step(m, stream, c);
 }
 
 static void ensure_staging(Model& m, uint32_t batch) {
@@ -904,9 +948,6 @@ static bool host_ptr_is_pinned(Model& m, const void* ptr) {
 	if (pinned) m.known_pinned[m.known_pinned_next++ % 4] = ptr;
 	return pinned;
 }
-
-static void dp_training_step(Model& m, cudaStream_t stream, uint32_t shard_batch, uint32_t global_batch, const float* x, const float* y);
-static void dp_reduce_loss(Model& m, cudaStream_t stream);
 
 // Enqueue one training step on HOST buffers and return at once: host->device copies on the copy stream (they overlap the kernels
 // of the step submitted before), the step on the model's compute stream (the binning pass starts when the positions have
@@ -1014,85 +1055,6 @@ static std::string make_hyperparams(const Model& m) {
 }
 
 }  // namespace tcnnb
-
-namespace tcnnb {
-__global__ void half_to_float_kernel(uint64_t n, const __half* __restrict__ in, float* __restrict__ out) {
-	const uint64_t i = threadIdx.x + (uint64_t)blockIdx.x * blockDim.x;
-	if (i < n) out[i] = (float)in[i];
-}
-
-__global__ void half_accumulate_kernel(uint64_t n, const __half* __restrict__ in, __half* __restrict__ inout) {
-	const uint64_t i = threadIdx.x + (uint64_t)blockIdx.x * blockDim.x;
-	if (i < n) inout[i] = __hadd(inout[i], in[i]);
-}
-
-// tcnn::GradientMode (object.h:116-120)
-enum GradientMode : int { GRADIENT_IGNORE = 0, GRADIENT_OVERWRITE = 1, GRADIENT_ACCUMULATE = 2 };
-
-// Trainer::training_step with all of its arguments (trainer.h:254-357): the fused kernel or the general path with the loss weighted by
-// `data_pdf`, or with the caller's `ext_dL_dy` (fp16 [batch][padded_output_width], already x loss scale) in place of the loss; the
-// gradients overwrite, add onto or leave alone the trainer's buffer; `dL_dinput` (fp32 [batch][n_in]) is overwritten. The optimizer
-// step, when asked for, comes last: the input gradient reads the parameters the step used.
-static void training_step_ex(Model& m, cudaStream_t stream, uint32_t batch, const float* x, const float* y, const float* data_pdf, bool run_optimizer, float* dL_dinput,
-                             bool use_inference_params, int mode, const __half* ext_dL_dy) {
-	if (m.module_only) throw std::runtime_error("this handle was created with tcnnb_module_create: use the tcnnb_module_* calls.");
-	if (m.dp) throw std::runtime_error("training_step_ex: data-parallel handles train with tcnnb_dp_training_step.");
-	if (mode != GRADIENT_IGNORE && mode != GRADIENT_OVERWRITE && mode != GRADIENT_ACCUMULATE) {
-		throw std::runtime_error("training_step_ex: param_gradients_mode must be 0 (Ignore), 1 (Overwrite) or 2 (Accumulate).");
-	}
-	if (!ext_dL_dy && !y) throw std::runtime_error("training_step: target is null and no external_dL_dy replaces the loss.");
-	if (!x) throw std::runtime_error("training_step: input is null.");
-	check_batch(batch);
-	if (ext_dL_dy) data_pdf = nullptr;  // the loss is not evaluated (trainer.h:127-131)
-	const __half* params = use_inference_params ? m.inference_params() : m.params_fp16;
-	const uint32_t n_mlp = m.mlp.n_params;
-	if (mode == GRADIENT_ACCUMULATE && !m.mlp_grads_in_accum && n_mlp) {
-		// the network's gradients are the fp16 values in the buffer (tcnnb_param_gradients materialised them): the fp32 sums continue
-		// from there
-		half_to_float_kernel<<<(n_mlp + 255) / 256, 256, 0, stream>>>(n_mlp, m.grads_fp16, m.dw_accum.ptr);
-		TCNNB_CUDA_CHECK(cudaGetLastError());
-		++g_kernel_launches;
-		m.mlp_grads_in_accum = true;
-	}
-	if (mode != GRADIENT_OVERWRITE) m.grads_scratch.resize(m.n_params_padded);
-	if (m.use_general()) {
-		if (ext_dL_dy) TCNNB_CUDA_CHECK(cudaMemsetAsync(m.scalars.ptr, 0, sizeof(float), stream));
-		// the general path overwrites the table gradients it computes: Accumulate adds them onto the buffer afterwards
-		__half* const grads = mode == GRADIENT_OVERWRITE ? m.grads_fp16 : m.grads_scratch.ptr;
-		general_backward_pass(m, stream, batch, batch, x, y, params, grads, ext_dL_dy, dL_dinput, mode != GRADIENT_IGNORE, data_pdf, mode != GRADIENT_OVERWRITE);
-		if (mode == GRADIENT_ACCUMULATE && m.plan.n_params) {
-			half_accumulate_kernel<<<(uint32_t)((m.plan.n_params + 255) / 256), 256, 0, stream>>>(m.plan.n_params, grads + n_mlp, m.grads_fp16 + n_mlp);
-			TCNNB_CUDA_CHECK(cudaGetLastError());
-			++g_kernel_launches;
-		}
-	} else {
-		if (dL_dinput && single_encoding(m.plan, FEAT_IDENTITY)) {
-			throw std::runtime_error("training_step: input gradients through an Identity encoding are not built for configurations the fused kernel runs; the general path (e.g. n_neurons > 64) computes them.");
-		}
-		ModuleIO io;
-		io.params = params;
-		io.dL_doutput = ext_dL_dy;
-		io.data_pdf = data_pdf;
-		io.accumulate = mode != GRADIENT_OVERWRITE;
-		io.grads = m.grads_fp16;
-		if (mode == GRADIENT_IGNORE) {
-			// the kernel still scatters: into scratch (trainer.h:338 hands the reference's a null gradient buffer). The scratch is never
-			// zeroed, so its sums keep growing over Ignore steps; nothing reads it.
-			io.grads = m.grads_scratch.ptr;
-			m.dw_scratch.resize(n_mlp);
-			io.dw_accum = m.dw_scratch.ptr;
-		}
-		if (dL_dinput) {
-			m.denc_scratch.resize(std::max(m.denc_scratch.n, (size_t)batch * 64));
-			io.dL_dencoded = m.denc_scratch.ptr;
-		}
-		training_step(m, stream, batch, batch, x, y, false, nullptr, &io);
-		if (dL_dinput) plan_input_gradient(m.plan, stream, batch, x, params + n_mlp, m.denc_scratch.ptr, 64, dL_dinput, 1.0f);
-	}
-	if (run_optimizer) optimizer_step(m, stream);
-}
-}  // namespace tcnnb
-
 
 // ==================================================================================================================
 // C ABI
@@ -1308,7 +1270,10 @@ int tcnnb_loss(tcnnb_model* m, tcnnb_stream stream, float* loss_out) {
 
 int tcnnb_inference(tcnnb_model* m, tcnnb_stream stream, uint32_t batch_size, const float* input_dev, float* output_dev) {
 	TCNNB_API_BEGIN
-	inference(m->impl, (cudaStream_t)stream, batch_size, input_dev, output_dev);
+	Model& mm = m->impl;
+	check_batch(batch_size);
+	check_trainer(mm);
+	forward(mm, (cudaStream_t)stream, batch_size, input_dev, mm.inference_params(), nullptr, output_dev);
 	TCNNB_API_END
 }
 
@@ -1346,12 +1311,13 @@ int tcnnb_inference_host(tcnnb_model* m, uint32_t batch_size, const float* input
 	TCNNB_API_BEGIN
 	Model& mm = m->impl;
 	check_batch(batch_size);
+	check_trainer(mm);
 	ensure_staging(mm, batch_size);
 	cudaStream_t s = mm.own_stream;
 	const size_t n_x = (size_t)batch_size * mm.n_in, n_y = (size_t)batch_size * mm.n_out;
 	std::memcpy(mm.pinned, input_host, n_x * sizeof(float));
 	TCNNB_CUDA_CHECK(cudaMemcpyAsync(mm.stage_in.ptr, mm.pinned, n_x * sizeof(float), cudaMemcpyHostToDevice, s));
-	inference(mm, s, batch_size, mm.stage_in.ptr, mm.stage_out.ptr);
+	forward(mm, s, batch_size, mm.stage_in.ptr, mm.inference_params(), nullptr, mm.stage_out.ptr);
 	TCNNB_CUDA_CHECK(cudaMemcpyAsync(mm.pinned + n_x, mm.stage_out.ptr, n_y * sizeof(float), cudaMemcpyDeviceToHost, s));
 	TCNNB_CUDA_CHECK(cudaStreamSynchronize(s));
 	std::memcpy(output_host, mm.pinned + n_x, n_y * sizeof(float));
@@ -1566,15 +1532,16 @@ int tcnnb_module_initialize_params(tcnnb_model* m, uint64_t seed, float* params_
 
 int tcnnb_module_inference(tcnnb_model* m, tcnnb_stream stream, uint32_t n_elements, const float* input_dev, void* output_dev, const void* params_dev) {
 	TCNNB_API_BEGIN
-	module_forward(m->impl, (cudaStream_t)stream, n_elements, input_dev, output_dev, params_dev);
+	check_batch(n_elements);
+	check_module_ptr(params_dev, "params");
+	check_module_ptr(output_dev, "output");
+	forward(m->impl, (cudaStream_t)stream, n_elements, input_dev, (const __half*)params_dev, (__half*)output_dev, nullptr);
 	TCNNB_API_END
 }
 
 int tcnnb_module_forward(tcnnb_model* m, tcnnb_stream stream, uint32_t n_elements, const float* input_dev, void* output_dev, const void* params_dev, int prepare_input_gradients) {
-	TCNNB_API_BEGIN
 	(void)prepare_input_gradients;  // nothing to prepare: backward recomputes the forward pass, including d(encoded)/d(position)
-	module_forward(m->impl, (cudaStream_t)stream, n_elements, input_dev, output_dev, params_dev);
-	TCNNB_API_END
+	return tcnnb_module_inference(m, stream, n_elements, input_dev, output_dev, params_dev);
 }
 
 int tcnnb_module_backward(tcnnb_model* m, tcnnb_stream stream, uint32_t n_elements, float* dL_dinput_dev, const void* dL_doutput_dev, void* dL_dparams_dev, const float* input_dev,
