@@ -112,6 +112,34 @@ int tcnnb_training_step(tcnnb_model* m, tcnnb_stream stream, uint32_t batch_size
  * external_dL_dy, batches that are not a multiple of tcnnb_batch_size_granularity(). */
 int tcnnb_training_step_ex(tcnnb_model* m, tcnnb_stream stream, uint32_t batch_size, const float* input_dev, const float* target_dev, const float* data_pdf_dev,
                            int run_optimizer, float* dL_dinput_dev, int use_inference_params, int param_gradients_mode, const void* external_dL_dy_dev);
+/* ---- Trainer::forward / Trainer::backward (trainer.h:89-153): a training step split around a ForwardContext whose buffers the
+ * caller owns. The library keeps nothing between the two calls; backward recomputes the forward pass.
+ * tcnnb_forward: trainer->forward(stream, loss_scale, input, target, data_pdf, use_inference_params, prepare_input_gradients,
+ *                external_dL_dy) (trainer.h:97-139). Device pointers.
+ *   output_dev          fp16 [batch][padded_output_width], 16-byte aligned, required: the predictions (ctx.output), with the
+ *                       tcnnb_params_inference weights when use_inference_params != 0.
+ *   loss_values_dev     fp32 [batch][padded_output_width] (ctx.L): the loss per element, padding columns 0. May be null.
+ *   dL_doutput_dev      fp16 [batch][padded_output_width], 16-byte aligned (ctx.dL_doutput): d(loss)/d(output) x the loss scale,
+ *                       padding columns 0 -- the loss's own gradient; backward passes it through the output activation. May be null.
+ *   target_dev, data_pdf_dev  as in tcnnb_training_step_ex; data_pdf_dev may be null.
+ *   external_dL_dy_dev  when non-null the loss is not evaluated: target and pdf are not read, loss_values_dev is left untouched (the
+ *                       reference leaves L unfilled), and dL_doutput_dev must be null -- the caller's buffer is the context's
+ *                       dL_doutput, handed to tcnnb_backward. Only its presence is read here.
+ *   prepare_input_gradients  accepted; nothing to prepare.
+ * tcnnb_backward: trainer->backward(stream, ctx, input, dL_dinput, use_inference_params, param_gradients_mode) (trainer.h:147-153).
+ *   Back-propagates dL_doutput_dev (fp16 [batch][padded_output_width], read when the call runs, so writes between forward and backward
+ *   count) through the output activation into the trainer's gradient buffer, with param_gradients_mode and dL_dinput_dev as in
+ *   tcnnb_training_step_ex. output_dev is accepted and not read. The optimizer does not run: tcnnb_optimizer_step does.
+ * Rejected like tcnnb_training_step_ex: handles of tcnnb_module_create, data-parallel handles, batches that are not a multiple of
+ * tcnnb_batch_size_granularity(), a null target without external_dL_dy, param_gradients_mode outside 0..2; and a non-null
+ * dL_doutput_dev together with external_dL_dy_dev. */
+int tcnnb_forward(tcnnb_model* m, tcnnb_stream stream, uint32_t batch_size, const float* input_dev, const float* target_dev, const float* data_pdf_dev, int use_inference_params,
+                  int prepare_input_gradients, const void* external_dL_dy_dev, void* output_dev, float* loss_values_dev, void* dL_doutput_dev);
+int tcnnb_backward(tcnnb_model* m, tcnnb_stream stream, uint32_t batch_size, const float* input_dev, const void* output_dev, const void* dL_doutput_dev, float* dL_dinput_dev,
+                   int use_inference_params, int param_gradients_mode);
+/* reduce_sum(values, n, stream) (reduce_sum.h:132-146): the fp32 sum of a device array, e.g. trainer->loss(ctx) of a forward context
+ * (the sum of ctx.L). Synchronises the stream. */
+int tcnnb_reduce_sum(tcnnb_stream stream, const float* values_dev, uint64_t n_elements, float* sum_out);
 /* Data-parallel variant: this rank's shard of a global batch; the loss is normalised over global_batch_size
  * (loss n_total, relative_l2.h:62) so that gradient sums over ranks equal the single-GPU gradients. */
 int tcnnb_training_step_shard(tcnnb_model* m, tcnnb_stream stream, uint32_t shard_batch_size, uint32_t global_batch_size, const float* input_dev, const float* target_dev, int run_optimizer);

@@ -104,13 +104,21 @@ private:
 	std::shared_ptr<detail::ModelHandle> m_model;
 };
 
-/* trainer.h:89-95; here it only marks "a step has been enqueued" -- the loss accumulator lives in the model */
-struct ForwardContext {};
-
 template <typename T, typename PARAMS_T, typename COMPUTE_T = PARAMS_T>
 class Trainer {
 public:
-	using Context = ForwardContext;
+	/* trainer.h:89-95. Filled by forward(): output, dL_doutput and L are padded_output_width x batch, column-major (sample-contiguous);
+	 * L holds the loss per element (padding rows 0; zero with external_dL_dy) and dL_doutput the loss gradient x loss scale, or views the
+	 * caller's external_dL_dy.
+	 * perturbed_output stays empty (perturbation_sigma is not built) and model_ctx is empty: backward recomputes the forward pass.
+	 * A context of training_step() is empty; its loss is kept by the model. */
+	struct ForwardContext : public Context {
+		GPUMatrix<COMPUTE_T> perturbed_output;
+		GPUMatrix<COMPUTE_T> output;
+		GPUMatrix<COMPUTE_T> dL_doutput;
+		GPUMatrix<float> L;
+		std::unique_ptr<Context> model_ctx;
+	};
 
 	/* trainer.h:51-58 */
 	Trainer(std::shared_ptr<NetworkWithInputEncoding<COMPUTE_T>> model, std::shared_ptr<Optimizer<PARAMS_T>> optimizer, std::shared_ptr<Loss<COMPUTE_T>> loss, uint32_t seed = 1337)
@@ -123,14 +131,14 @@ public:
 	/* trainer.h:254-357. Matrices are n_dims x batch, column-major: input, target, data_pdf and dL_dinput fp32, external_dL_dy
 	 * COMPUTE_T (fp16) padded_output_width x batch and already multiplied by the loss scale. With external_dL_dy the loss is not
 	 * evaluated (target and data_pdf are not read) and loss() returns 0. */
-	std::unique_ptr<Context> training_step(cudaStream_t stream, const GPUMatrixDynamic<T>& input, const GPUMatrixDynamic<float>& target, const GPUMatrixDynamic<float>* data_pdf = nullptr,
+	std::unique_ptr<ForwardContext> training_step(cudaStream_t stream, const GPUMatrixDynamic<T>& input, const GPUMatrixDynamic<float>& target, const GPUMatrixDynamic<float>* data_pdf = nullptr,
 	                                       bool run_optimizer = true, GPUMatrixDynamic<T>* dL_dinput = nullptr, bool use_inference_params = false,
 	                                       GradientMode param_gradients_mode = GradientMode::Overwrite, const GPUMatrixDynamic<COMPUTE_T>* external_dL_dy = nullptr) {
 		if (!data_pdf && !dL_dinput && !use_inference_params && param_gradients_mode == GradientMode::Overwrite && !external_dL_dy) {
 			if (input.n() != target.n()) throw std::runtime_error{"training_step: input and target batch sizes differ"};
 			if (input.layout() != CM || target.layout() != CM) throw std::runtime_error{"training_step: column-major (sample-contiguous) matrices only"};
 			TCNNB_CHECK_THROW(tcnnb_training_step(m_handle->m, (tcnnb_stream)stream, input.n(), input.data(), target.data(), run_optimizer ? 1 : 0));
-			return std::make_unique<Context>();
+			return std::make_unique<ForwardContext>();
 		}
 		const uint32_t batch_size = input.n();
 		if (input.layout() != CM) throw std::runtime_error{"training_step: column-major (sample-contiguous) matrices only"};
@@ -154,22 +162,79 @@ public:
 		TCNNB_CHECK_THROW(tcnnb_training_step_ex(m_handle->m, (tcnnb_stream)stream, batch_size, input.data(), external_dL_dy ? nullptr : target.data(),
 		                                         external_dL_dy || !data_pdf ? nullptr : data_pdf->data(), run_optimizer ? 1 : 0, dL_dinput ? dL_dinput->data() : nullptr,
 		                                         use_inference_params ? 1 : 0, (int)param_gradients_mode, external_dL_dy ? external_dL_dy->data() : nullptr));
-		return std::make_unique<Context>();
+		return std::make_unique<ForwardContext>();
 	}
-	std::unique_ptr<Context> training_step(const GPUMatrixDynamic<T>& input, const GPUMatrixDynamic<float>& target, const GPUMatrixDynamic<float>* data_pdf = nullptr,
+	std::unique_ptr<ForwardContext> training_step(const GPUMatrixDynamic<T>& input, const GPUMatrixDynamic<float>& target, const GPUMatrixDynamic<float>* data_pdf = nullptr,
 	                                       bool run_optimizer = true, GPUMatrixDynamic<T>* dL_dinput = nullptr, bool use_inference_params = false,
 	                                       GradientMode param_gradients_mode = GradientMode::Overwrite, const GPUMatrixDynamic<COMPUTE_T>* external_dL_dy = nullptr) {
 		return training_step(nullptr, input, target, data_pdf, run_optimizer, dL_dinput, use_inference_params, param_gradients_mode, external_dL_dy);
 	}
 
+	/* trainer.h:97-145: the predictions, and unless external_dL_dy is given the loss values and loss gradient, of one batch. The loss
+	 * scale is the trainer's own (default_loss_scale, 128). With external_dL_dy, ctx->dL_doutput is a view of the caller's matrix: what the
+	 * caller writes there before backward() is what backward() propagates. */
+	std::unique_ptr<ForwardContext> forward(cudaStream_t stream, const float loss_scale, const GPUMatrixDynamic<T>& input, const GPUMatrix<float>& target,
+	                                        const GPUMatrix<float>* data_pdf = nullptr, bool use_inference_params = false, bool prepare_input_gradients = false,
+	                                        const GPUMatrix<COMPUTE_T>* external_dL_dy = nullptr) {
+		const uint32_t batch_size = input.n(), padded = m_model->padded_output_width();
+		if (loss_scale != tcnnb_default_loss_scale()) throw std::runtime_error{"forward: the trainer's loss scale is default_loss_scale (128)"};
+		if (input.layout() != CM) throw std::runtime_error{"forward: column-major (sample-contiguous) matrices only"};
+		auto ctx = std::make_unique<ForwardContext>();
+		ctx->output = GPUMatrix<COMPUTE_T>{padded, batch_size};
+		ctx->model_ctx = std::make_unique<Context>();
+		ctx->L = GPUMatrix<float>{padded, batch_size};
+		if (external_dL_dy) {  /* trainer.h:127-131 */
+			CHECK_THROW(external_dL_dy->m() == padded);
+			CHECK_THROW(external_dL_dy->n() == batch_size);
+			ctx->dL_doutput = GPUMatrix<COMPUTE_T>{external_dL_dy->data(), padded, batch_size};
+			ctx->L.memset_async(stream, 0);  /* no loss is evaluated: loss(ctx) is 0, as for training_step with external_dL_dy */
+		} else {  /* trainer.h:133-138 */
+			CHECK_THROW(input.n() == target.n());
+			CHECK_THROW(m_model->output_width() == target.m());
+			CHECK_THROW(!data_pdf || (data_pdf->m() == target.m() && data_pdf->n() == batch_size));
+			ctx->dL_doutput = GPUMatrix<COMPUTE_T>{padded, batch_size};
+		}
+		TCNNB_CHECK_THROW(tcnnb_forward(m_handle->m, (tcnnb_stream)stream, batch_size, input.data(), external_dL_dy ? nullptr : target.data(),
+		                                external_dL_dy || !data_pdf ? nullptr : data_pdf->data(), use_inference_params ? 1 : 0, prepare_input_gradients ? 1 : 0,
+		                                external_dL_dy ? external_dL_dy->data() : nullptr, ctx->output.data(), ctx->L.data(), external_dL_dy ? nullptr : ctx->dL_doutput.data()));
+		return ctx;
+	}
+	std::unique_ptr<ForwardContext> forward(const float loss_scale, const GPUMatrixDynamic<T>& input, const GPUMatrix<float>& target, const GPUMatrix<float>* data_pdf = nullptr,
+	                                        bool use_inference_params = false, bool prepare_input_gradients = false, const GPUMatrix<COMPUTE_T>* external_dL_dy = nullptr) {
+		return forward(nullptr, loss_scale, input, target, data_pdf, use_inference_params, prepare_input_gradients, external_dL_dy);
+	}
+
+	/* trainer.h:147-153: back-propagates ctx.dL_doutput into the gradient buffer (GradientMode as in training_step); no optimizer step */
+	void backward(cudaStream_t stream, const ForwardContext& ctx, const GPUMatrixDynamic<T>& input, GPUMatrixDynamic<T>* dL_dinput = nullptr, bool use_inference_params = false,
+	              GradientMode param_gradients_mode = GradientMode::Overwrite) {
+		const uint32_t batch_size = input.n();
+		if (input.layout() != CM) throw std::runtime_error{"backward: column-major (sample-contiguous) matrices only"};
+		CHECK_THROW(ctx.dL_doutput.m() == m_model->padded_output_width());
+		CHECK_THROW(ctx.dL_doutput.n() == batch_size);
+		if (dL_dinput) {
+			CHECK_THROW(dL_dinput->m() == m_model->input_width());
+			CHECK_THROW(dL_dinput->n() == batch_size);
+			if (dL_dinput->layout() != CM) throw std::runtime_error{"backward: column-major (sample-contiguous) matrices only"};
+		}
+		TCNNB_CHECK_THROW(tcnnb_backward(m_handle->m, (tcnnb_stream)stream, batch_size, input.data(), ctx.output.data(), ctx.dL_doutput.data(), dL_dinput ? dL_dinput->data() : nullptr,
+		                                 use_inference_params ? 1 : 0, (int)param_gradients_mode));
+	}
+	void backward(const ForwardContext& ctx, const GPUMatrixDynamic<T>& input, GPUMatrixDynamic<T>* dL_dinput = nullptr, bool use_inference_params = false,
+	              GradientMode param_gradients_mode = GradientMode::Overwrite) {
+		backward(nullptr, ctx, input, dL_dinput, use_inference_params, param_gradients_mode);
+	}
+
 	void optimizer_step(cudaStream_t stream, float /*loss_scale*/) { TCNNB_CHECK_THROW(tcnnb_optimizer_step(m_handle->m, (tcnnb_stream)stream)); } /* trainer.h:155-157 */
 
-	/* trainer.h:372-378: sum of the per-element losses of the last step (device -> host, synchronises the stream) */
-	float loss(cudaStream_t stream, const Context&) const {
+	/* trainer.h:372-378: the sum of ctx.L for a context of forward(); for a context of training_step(), the sum of the per-element
+	 * losses of the last step. Device -> host, synchronises the stream. */
+	float loss(cudaStream_t stream, const ForwardContext& ctx) const {
 		float v = 0;
-		TCNNB_CHECK_THROW(tcnnb_loss(m_handle->m, (tcnnb_stream)stream, &v));
+		if (ctx.L.data()) TCNNB_CHECK_THROW(tcnnb_reduce_sum((tcnnb_stream)stream, ctx.L.data(), ctx.L.n_elements(), &v));
+		else TCNNB_CHECK_THROW(tcnnb_loss(m_handle->m, (tcnnb_stream)stream, &v));
 		return v;
 	}
+	float loss(const ForwardContext& ctx) const { return loss(nullptr, ctx); }
 
 	/* trainer.h:442-482 + optimizers/adam.h:303-325: the reference's snapshot schema (nlohmann binary values; instant-ngp stores it as
 	 * msgpack): {"n_params", "params_type": "__half", "params_binary", "optimizer": {"current_step", "base_learning_rate",

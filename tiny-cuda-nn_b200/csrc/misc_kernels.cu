@@ -8,6 +8,8 @@
 
 #include "fused_common.cuh"
 
+#include <algorithm>
+
 namespace tcnnb {
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -245,12 +247,28 @@ __global__ void mlp_grad_finalize_kernel(uint32_t n, float* __restrict__ dw_accu
 	}
 }
 
-// ---- loss on its own (general, unfused training path): prediction rows [batch][stride] fp16 + targets [batch][n_out] fp32 ->
-// dL/d(output) rows (x loss_scale, through the output activation's transfer, padding columns zero), per-element values, sum.
-// Same expressions as the fused kernel's output epilogue (fused_common.cuh loss_element).
+// Adds `value` of every thread of the block (256 threads) onto *sum with ONE atomic per block (a per-warp atomic on a single word
+// serialises the whole kernel). Every thread of the block must call it.
+__device__ __forceinline__ void block_sum_add(float value, float* sum) {
+	__shared__ float warp_sums[8];
+#pragma unroll
+	for (uint32_t o = 16; o > 0; o >>= 1) value += __shfl_xor_sync(0xFFFFFFFFu, value, o);
+	if ((threadIdx.x & 31u) == 0) warp_sums[threadIdx.x >> 5] = value;
+	__syncthreads();
+	if (threadIdx.x == 0 && sum) {
+		float total = 0.0f;
+		for (uint32_t w = 0; w < blockDim.x / 32; ++w) total += warp_sums[w];
+		if (total != 0.0f) atomicAdd(sum, total);
+	}
+}
+
+// ---- loss on its own (general, unfused training path; Trainer::forward): prediction rows [batch][stride] fp16 + targets [batch][n_out]
+// fp32 -> dL/d(output) rows (x loss_scale, through the output activation's transfer, padding columns zero), per-element values
+// [batch][values_stride] (columns from n_out on zero), sum. Same expressions as the fused kernel's output epilogue (fused_common.cuh
+// loss_element).
 __global__ void loss_kernel(uint32_t loss_type, uint32_t out_act, uint32_t batch, uint32_t n_out, uint32_t stride, float loss_scale, float n_total, const __half* __restrict__ prediction,
                             const float* __restrict__ targets, const float* __restrict__ data_pdf, __half* __restrict__ dL_dy, float* __restrict__ loss_values,
-                            float* __restrict__ loss_sum) {
+                            uint32_t values_stride, float* __restrict__ loss_sum) {
 	pdl_wait();
 	pdl_launch_dependents();
 	// one thread per (sample, group of 8 output columns): 16-byte loads / stores of the fp16 rows
@@ -266,31 +284,28 @@ __global__ void loss_kernel(uint32_t loss_type, uint32_t out_act, uint32_t batch
 #pragma unroll
 		for (uint32_t k = 0; k < 8; ++k) {
 			const uint32_t q = q0 + k;
-			float gq = 0.0f;
+			float gq = 0.0f, value = 0.0f;
 			if (q < n_out) {
-				float value, grad;
+				float grad;
 				const size_t t = (size_t)sample * n_out + q;
 				if (data_pdf) fused::loss_element_pdf(loss_type, __half2float(y[k]), targets[t], data_pdf[t], n_total, luminance, value, grad);
 				else fused::loss_element(loss_type, __half2float(y[k]), targets[t], n_total, luminance, value, grad);
 				gq = loss_scale * grad / n_total;
 				value_sum += value;
-				if (loss_values) loss_values[(size_t)sample * n_out + q] = value;
 			}
+			if (loss_values && q < values_stride) loss_values[(size_t)sample * values_stride + q] = value;
 			dy[k] = fused::act_bwd_h(out_act, __float2half_rn(gq), y[k]);
 		}
-		*reinterpret_cast<uint4*>(dL_dy + (size_t)sample * stride + q0) = *reinterpret_cast<const uint4*>(dy);
+		if (dL_dy) *reinterpret_cast<uint4*>(dL_dy + (size_t)sample * stride + q0) = *reinterpret_cast<const uint4*>(dy);
 	}
-	// block sum -> ONE atomic per block (a per-warp atomic on the single loss word serialises the whole kernel)
-	__shared__ float warp_sums[8];
-#pragma unroll
-	for (uint32_t o = 16; o > 0; o >>= 1) value_sum += __shfl_xor_sync(0xFFFFFFFFu, value_sum, o);
-	if ((threadIdx.x & 31u) == 0) warp_sums[threadIdx.x >> 5] = value_sum;
-	__syncthreads();
-	if (threadIdx.x == 0 && loss_sum) {
-		float total = 0.0f;
-		for (uint32_t w = 0; w < blockDim.x / 32; ++w) total += warp_sums[w];
-		if (total != 0.0f) atomicAdd(loss_sum, total);
-	}
+	block_sum_add(value_sum, loss_sum);
+}
+
+// reduce_sum (reduce_sum.h:132-146): grid-stride partial sums, one atomic per block onto *sum (zeroed by the launcher)
+__global__ void reduce_sum_kernel(uint64_t n, const float* __restrict__ values, float* __restrict__ sum) {
+	float v = 0.0f;
+	for (uint64_t i = threadIdx.x + (uint64_t)blockIdx.x * blockDim.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) v += values[i];
+	block_sum_add(v, sum);
 }
 
 // dL/d(output) of a caller (Network::backward, fully_fused_mlp.cu:755-762) through the output activation's transfer.
@@ -486,10 +501,17 @@ cudaError_t launch_mlp_grad_finalize(cudaStream_t stream, uint32_t n, float* dw_
 }
 
 cudaError_t launch_loss(cudaStream_t stream, uint32_t loss_type, uint32_t output_activation, uint32_t batch, uint32_t n_out, uint32_t stride, float loss_scale, uint32_t n_total,
-                        const __half* prediction, const float* targets, const float* data_pdf, __half* dL_dy, float* loss_values, float* loss_sum) {
-	if ((uint64_t)batch * stride >= (1ull << 32) || stride % 8 != 0) return cudaErrorInvalidValue;
+                        const __half* prediction, const float* targets, const float* data_pdf, __half* dL_dy, float* loss_values, uint32_t values_stride, float* loss_sum) {
+	if ((uint64_t)batch * stride >= (1ull << 32) || stride % 8 != 0 || values_stride < n_out || values_stride > stride) return cudaErrorInvalidValue;
 	return launch_pdl(loss_kernel, blocks_for(batch * (stride / 8), 256), 256, 0, stream, loss_type, output_activation, batch, n_out, stride, loss_scale, (float)n_total, prediction, targets,
-	                  data_pdf, dL_dy, loss_values, loss_sum);
+	                  data_pdf, dL_dy, loss_values, values_stride, loss_sum);
+}
+
+cudaError_t launch_reduce_sum(cudaStream_t stream, uint64_t n, const float* values, float* sum) {
+	cudaError_t e = cudaMemsetAsync(sum, 0, sizeof(float), stream);
+	if (e != cudaSuccess || n == 0) return e;
+	reduce_sum_kernel<<<(uint32_t)std::min<uint64_t>((n + 255) / 256, 1024), 256, 0, stream>>>(n, values, sum);
+	return cudaGetLastError();
 }
 
 cudaError_t launch_activation_backward_output(cudaStream_t stream, uint32_t activation, uint64_t n, const __half* grad, const __half* forward_output, __half* out) {

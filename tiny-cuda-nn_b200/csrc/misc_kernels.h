@@ -42,10 +42,13 @@ cudaError_t launch_widen_steps(cudaStream_t stream, uint64_t n, const uint16_t* 
 cudaError_t launch_narrow_steps(cudaStream_t stream, uint64_t n, const uint32_t* in, uint16_t* out);
 cudaError_t launch_mlp_grad_finalize(cudaStream_t stream, uint32_t n, float* dw_accum, __half* gradients);
 
-// General (unfused) training path: loss + dL/d(output) from fp16 prediction rows [batch][stride]; data_pdf ([batch][n_out], divides the
-// loss as in losses/*.h), loss_values and loss_sum may be null.
+// General (unfused) training path and Trainer::forward: loss + dL/d(output) from fp16 prediction rows [batch][stride]; data_pdf ([batch][n_out],
+// divides the loss as in losses/*.h), dL_dy, loss_values ([batch][values_stride], n_out <= values_stride <= stride, columns from n_out on
+// zero) and loss_sum may be null.
 cudaError_t launch_loss(cudaStream_t stream, uint32_t loss_type, uint32_t output_activation, uint32_t batch, uint32_t n_out, uint32_t stride, float loss_scale, uint32_t n_total,
-                        const __half* prediction, const float* targets, const float* data_pdf, __half* dL_dy, float* loss_values, float* loss_sum);
+                        const __half* prediction, const float* targets, const float* data_pdf, __half* dL_dy, float* loss_values, uint32_t values_stride, float* loss_sum);
+// *sum = the fp32 sum of values[0, n) (reduce_sum.h:132-146), stream-ordered.
+cudaError_t launch_reduce_sum(cudaStream_t stream, uint64_t n, const float* values, float* sum);
 // out = grad * f'(.) of the output activation, expressed through the forward output (element-wise, fp16).
 cudaError_t launch_activation_backward_output(cudaStream_t stream, uint32_t activation, uint64_t n, const __half* grad, const __half* forward_output, __half* out);
 

@@ -651,7 +651,7 @@ static void general_backward(Model& m, cudaStream_t stream, const BackwardCall& 
 		grow(m.g_dy, (size_t)c.batch * mlp.padded_out_width);
 		__half* const dy_rows = (m.taps.dL_doutput && mlp.padded_out_width == 16) ? (__half*)m.taps.dL_doutput : m.g_dy.ptr;
 		TCNNB_CUDA_CHECK(launch_loss(stream, m.loss_type, mlp.output_activation, c.batch, m.n_out, mlp.padded_out_width, m.loss_scale, c.loss_batch * m.n_out, out_rows, c.y,
-		                             c.data_pdf, dy_rows, m.taps.loss_values, m.scalars.ptr));
+		                             c.data_pdf, dy_rows, m.taps.loss_values, m.n_out, m.scalars.ptr));
 		++g_kernel_launches;
 		dL_doutput = dy_rows;
 	}
@@ -926,6 +926,27 @@ static void training_step_ex(Model& m, cudaStream_t stream, uint32_t batch, cons
 	c.dL_dinput = dL_dinput;
 	c.run_optimizer = run_optimizer;
 	backward_step(m, stream, c);
+}
+
+// Trainer::forward (trainer.h:97-139): the padded fp16 predictions of the inference launch, then -- unless the caller brings its own
+// dL/d(output) -- the loss on them: per-element values and dL/d(output) x loss scale, both [batch][padded_output_width] with zero
+// padding columns. The gradient is the loss's alone, as in the reference's context: the backward pass takes it through the output
+// activation like an external_dL_dy. Nothing is kept for the backward pass, which recomputes the forward.
+static void trainer_forward(Model& m, cudaStream_t stream, uint32_t batch, const float* x, const float* y, const float* data_pdf, bool use_inference_params, bool external_dL_dy,
+                            __half* output, float* loss_values, __half* dL_doutput) {
+	check_trainer(m);
+	if (m.dp) throw std::runtime_error("forward: data-parallel handles train with tcnnb_dp_training_step.");
+	if (!external_dL_dy && !y) throw std::runtime_error("forward: target is null and no external_dL_dy replaces the loss.");
+	if (external_dL_dy && dL_doutput) throw std::runtime_error("forward: with external_dL_dy the caller's buffer is dL_doutput; dL_doutput_dev must be null.");
+	if (!x) throw std::runtime_error("forward: input is null.");
+	if (!output || (uintptr_t)output % 16 != 0) throw std::runtime_error("forward: output must be a 16-byte aligned device array.");
+	if ((uintptr_t)dL_doutput % 16 != 0) throw std::runtime_error("forward: dL_doutput must be 16-byte aligned.");
+	check_batch(batch);
+	forward(m, stream, batch, x, use_inference_params ? m.inference_params() : m.params_fp16, output, nullptr);
+	if (external_dL_dy || (!loss_values && !dL_doutput)) return;
+	const uint32_t pad = m.mlp.padded_out_width;
+	TCNNB_CUDA_CHECK(launch_loss(stream, m.loss_type, ACT_NONE, batch, m.n_out, pad, m.loss_scale, batch * m.n_out, output, y, data_pdf, dL_doutput, loss_values, pad, nullptr));
+	++g_kernel_launches;
 }
 
 static void ensure_staging(Model& m, uint32_t batch) {
@@ -1237,6 +1258,42 @@ int tcnnb_training_step_ex(tcnnb_model* m, tcnnb_stream stream, uint32_t batch_s
 	TCNNB_API_BEGIN
 	training_step_ex(m->impl, (cudaStream_t)stream, batch_size, input_dev, target_dev, data_pdf_dev, run_optimizer != 0, dL_dinput_dev, use_inference_params != 0, param_gradients_mode,
 	                 (const __half*)external_dL_dy_dev);
+	TCNNB_API_END
+}
+
+int tcnnb_forward(tcnnb_model* m, tcnnb_stream stream, uint32_t batch_size, const float* input_dev, const float* target_dev, const float* data_pdf_dev, int use_inference_params,
+                  int prepare_input_gradients, const void* external_dL_dy_dev, void* output_dev, float* loss_values_dev, void* dL_doutput_dev) {
+	TCNNB_API_BEGIN
+	(void)prepare_input_gradients;  // nothing to prepare: backward recomputes the forward pass, including d(encoded)/d(position)
+	trainer_forward(m->impl, (cudaStream_t)stream, batch_size, input_dev, target_dev, data_pdf_dev, use_inference_params != 0, external_dL_dy_dev != nullptr, (__half*)output_dev,
+	                loss_values_dev, (__half*)dL_doutput_dev);
+	TCNNB_API_END
+}
+
+int tcnnb_backward(tcnnb_model* m, tcnnb_stream stream, uint32_t batch_size, const float* input_dev, const void* output_dev, const void* dL_doutput_dev, float* dL_dinput_dev,
+                   int use_inference_params, int param_gradients_mode) {
+	TCNNB_API_BEGIN
+	(void)output_dev;  // the forward pass is recomputed; the saved output is not needed
+	if (!dL_doutput_dev) throw std::runtime_error("backward: dL_doutput is null.");
+	training_step_ex(m->impl, (cudaStream_t)stream, batch_size, input_dev, nullptr, nullptr, false, dL_dinput_dev, use_inference_params != 0, param_gradients_mode,
+	                 (const __half*)dL_doutput_dev);
+	TCNNB_API_END
+}
+
+int tcnnb_reduce_sum(tcnnb_stream stream, const float* values_dev, uint64_t n_elements, float* sum_out) {
+	TCNNB_API_BEGIN
+	if (n_elements && !values_dev) throw std::runtime_error("reduce_sum: values are null.");
+	cudaStream_t s = (cudaStream_t)stream;
+	float* sum_dev = nullptr;
+	TCNNB_CUDA_CHECK(cudaMallocAsync(&sum_dev, sizeof(float), s));
+	float v = 0;
+	cudaError_t e = launch_reduce_sum(s, n_elements, values_dev, sum_dev);
+	if (e == cudaSuccess) e = cudaMemcpyAsync(&v, sum_dev, sizeof(float), cudaMemcpyDeviceToHost, s);
+	cudaFreeAsync(sum_dev, s);
+	TCNNB_CUDA_CHECK(e);
+	TCNNB_CUDA_CHECK(cudaStreamSynchronize(s));
+	if (n_elements) ++g_kernel_launches;
+	if (sum_out) *sum_out = v;
 	TCNNB_API_END
 }
 

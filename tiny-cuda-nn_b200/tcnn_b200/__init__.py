@@ -66,6 +66,9 @@ ABI = [
     ("tcnnb_set_learning_rate_factor", _int, [_vp, ctypes.c_float]),
     ("tcnnb_training_step", _int, [_vp, _vp, _u32, _vp, _vp, _int]),
     ("tcnnb_training_step_ex", _int, [_vp, _vp, _u32, _vp, _vp, _vp, _int, _vp, _int, _int, _vp]),
+    ("tcnnb_forward", _int, [_vp, _vp, _u32, _vp, _vp, _vp, _int, _int, _vp, _vp, _vp, _vp]),
+    ("tcnnb_backward", _int, [_vp, _vp, _u32, _vp, _vp, _vp, _vp, _int, _int]),
+    ("tcnnb_reduce_sum", _int, [_vp, _vp, _u64, _f32p]),
     ("tcnnb_training_step_shard", _int, [_vp, _vp, _u32, _u32, _vp, _vp, _int]),
     ("tcnnb_optimizer_step", _int, [_vp, _vp]),
     ("tcnnb_generate_random_uniform", _int, [_vp, ctypes.c_uint64, ctypes.c_uint64, ctypes.c_uint64, _vp, ctypes.c_float, ctypes.c_float]),
@@ -169,6 +172,23 @@ def _stream_handle(stream):
     return ctypes.c_void_p(stream.cuda_stream)
 
 
+def _tensor_ptr(t, dtype, shape):
+    """data_ptr() of a contiguous CUDA tensor of the given dtype and shape; None for None."""
+    if t is None:
+        return None
+    if not (t.is_cuda and t.dtype == dtype and t.is_contiguous() and tuple(t.shape) == shape):
+        raise ValueError(f"expected a contiguous CUDA {dtype} tensor of shape {shape}, got {t.dtype} {tuple(t.shape)}")
+    return t.data_ptr()
+
+
+class ForwardContext:
+    """Trainer::ForwardContext (trainer.h:89-95), as _Trainer.forward returns it: torch tensors `output`, `L` and `dL_doutput`,
+    each [B, padded_output_width]."""
+
+    def __init__(self, output, L, dL_doutput):
+        self.output, self.L, self.dL_doutput = output, L, dL_doutput
+
+
 class _Network:
     """NetworkWithInputEncoding surface: inference / n_params / padded_output_width."""
 
@@ -216,23 +236,52 @@ class _Trainer:
             assert targets.is_cuda and targets.dtype == torch.float32 and targets.is_contiguous()
             _check(load().tcnnb_training_step(m._h, _stream_handle(stream), inputs.shape[0], inputs.data_ptr(), targets.data_ptr(), int(run_optimizer)))
             return self
-        if gradient_mode not in self._GRADIENT_MODES:
-            raise ValueError(f"gradient_mode must be one of {sorted(self._GRADIENT_MODES)}, not {gradient_mode!r}")
         B = inputs.shape[0]
-
-        def ptr(t, dtype, shape):
-            if t is None:
-                return None
-            if not (t.is_cuda and t.dtype == dtype and t.is_contiguous() and tuple(t.shape) == shape):
-                raise ValueError(f"expected a contiguous CUDA {dtype} tensor of shape {shape}, got {t.dtype} {tuple(t.shape)}")
-            return t.data_ptr()
-
+        ptr = _tensor_ptr
         lib = load()
         n_out, pad = m.n_output_dims, lib.tcnnb_padded_output_width(m._h)
         _check(lib.tcnnb_training_step_ex(m._h, _stream_handle(stream), B, inputs.data_ptr(), ptr(targets, torch.float32, (B, n_out)),
                                           ptr(data_pdf, torch.float32, (B, n_out)), int(run_optimizer), ptr(dL_dinput, torch.float32, (B, m.n_input_dims)),
-                                          int(bool(use_inference_params)), self._GRADIENT_MODES[gradient_mode], ptr(external_dL_dy, torch.float16, (B, pad))))
+                                          int(bool(use_inference_params)), self._gradient_mode(gradient_mode), ptr(external_dL_dy, torch.float16, (B, pad))))
         return self
+
+    def _gradient_mode(self, mode):
+        if mode not in self._GRADIENT_MODES:
+            raise ValueError(f"gradient_mode must be one of {sorted(self._GRADIENT_MODES)}, not {mode!r}")
+        return self._GRADIENT_MODES[mode]
+
+    def forward(self, inputs, targets=None, data_pdf=None, use_inference_params=False, external_dL_dy=None, stream=None):
+        """trainer.forward (trainer.h:97-139): a ForwardContext with the predictions `output` [B, padded_output_width] fp16, the
+        per-element losses `L` [B, padded_output_width] fp32 and `dL_doutput` [B, padded_output_width] fp16 (loss gradient x loss scale;
+        padding columns 0). With `external_dL_dy` the loss is not evaluated: `L` stays zero and `dL_doutput` IS the caller's tensor,
+        which may be written before `backward` reads it."""
+        import torch
+
+        m = self._m
+        assert inputs.is_cuda and inputs.dtype == torch.float32 and inputs.is_contiguous()
+        B, lib = inputs.shape[0], load()
+        n_out, pad = m.n_output_dims, lib.tcnnb_padded_output_width(m._h)
+        ext = _tensor_ptr(external_dL_dy, torch.float16, (B, pad))
+        empty = torch.zeros if ext else torch.empty  # the loss kernel writes every element of L, padding included
+        ctx = ForwardContext(torch.empty(B, pad, dtype=torch.float16, device=inputs.device), empty(B, pad, dtype=torch.float32, device=inputs.device),
+                             external_dL_dy if ext else torch.empty(B, pad, dtype=torch.float16, device=inputs.device))
+        _check(lib.tcnnb_forward(m._h, _stream_handle(stream), B, inputs.data_ptr(), None if ext else _tensor_ptr(targets, torch.float32, (B, n_out)),
+                                 None if ext else _tensor_ptr(data_pdf, torch.float32, (B, n_out)), int(bool(use_inference_params)), 0, ext, ctx.output.data_ptr(),
+                                 ctx.L.data_ptr(), None if ext else ctx.dL_doutput.data_ptr()))
+        return ctx
+
+    def backward(self, ctx, inputs, dL_dinput=None, use_inference_params=False, gradient_mode="Overwrite", stream=None):
+        """trainer.backward (trainer.h:147-153): back-propagates ctx.dL_doutput as it is now into the gradient buffer ("Ignore",
+        "Overwrite" or "Accumulate"); `dL_dinput` [B, n_in] fp32 is overwritten with dL/d(input). No optimizer step."""
+        import torch
+
+        m = self._m
+        assert inputs.is_cuda and inputs.dtype == torch.float32 and inputs.is_contiguous()
+        B, lib = inputs.shape[0], load()
+        pad = lib.tcnnb_padded_output_width(m._h)
+        _check(lib.tcnnb_backward(m._h, _stream_handle(stream), B, inputs.data_ptr(), _tensor_ptr(ctx.output, torch.float16, (B, pad)),
+                                  _tensor_ptr(ctx.dL_doutput, torch.float16, (B, pad)), _tensor_ptr(dL_dinput, torch.float32, (B, m.n_input_dims)),
+                                  int(bool(use_inference_params)), self._gradient_mode(gradient_mode)))
 
     def training_step_shard(self, inputs, targets, global_batch_size, run_optimizer=False, stream=None):
         m = self._m
@@ -250,8 +299,13 @@ class _Trainer:
         _check(load().tcnnb_optimizer_step_ranges(self._m._h, _stream_handle(stream), n, b, c))
 
     def loss(self, ctx=None, stream=None):
+        """trainer.loss(ctx) (trainer.h:372-378): the sum of ctx.L for a context of forward(); otherwise the loss of the last
+        training step. Synchronises the stream."""
         out = ctypes.c_float(0)
-        _check(load().tcnnb_loss(self._m._h, _stream_handle(stream), ctypes.byref(out)))
+        if isinstance(ctx, ForwardContext):
+            _check(load().tcnnb_reduce_sum(_stream_handle(stream), ctx.L.data_ptr(), ctx.L.numel(), ctypes.byref(out)))
+        else:
+            _check(load().tcnnb_loss(self._m._h, _stream_handle(stream), ctypes.byref(out)))
         return out.value
 
     def n_params(self):
