@@ -5,9 +5,9 @@
 //   src/encoding.cu:132-150     create_encoding ("otype" dispatch, case-insensitive)  + grid.h:1726-1851 (grid JSON keys)
 //   src/network.cu:51-141       select_network / create_network
 //   src/loss.cu:82-90           create_loss
-//   src/optimizer.cu:50-80      create_optimizer + optimizers/adam.h:221-303 (Adam JSON keys)
 //   trainer.h:51-87,254-378     Trainer ctor / initialize_params / training_step / loss
 //   network_with_input_encoding.h:115-150  parameter layout [MLP | grid]
+// The optimizer (create_optimizer, src/optimizer.cu:50-80) is optimizer.cu's.
 // There is deliberately no fallback: unsupported configurations raise the error the caller sees via tcnnb_last_error().
 #include "../../include/tcnn_b200.h"
 
@@ -22,17 +22,16 @@
 #include "misc_kernels.h"
 #include "mlp_fused.h"
 #include "network_config.h"
+#include "optimizer.h"
 
 #include <dlfcn.h>
 #include <nccl.h>  // types and prototypes only: libnccl is resolved at run time (dlopen), single-GPU users never need it
 
 #include <algorithm>
 #include <atomic>
-#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
-#include <limits>
 #include <memory>
 #include <random>
 #include <stdexcept>
@@ -116,20 +115,7 @@ struct Model {
 	MlpConfig mlp;
 	uint32_t loss_type = LOSS_RELATIVE_L2;
 	std::string loss_name = "RelativeL2";
-	AdamParams adam;
-	uint32_t adam_step_count = 0;
-	struct {  // ExponentialDecay wrapper (optimizers/exponential_decay.h)
-		bool enabled = false;
-		float base = 0.1f, factor = 1.0f;
-		uint32_t interval = 10000, start = 10000, end = 10000000;
-	} lr_decay;
-	struct {  // Ema wrapper (optimizers/ema.h:46-200): exponential moving average of the working weights, used by inference
-		bool enabled = false, full_precision = false;
-		float decay = 0.99f;
-	} ema;
-	DeviceBuffer<__half> ema_fp16;  // Trainer::params_inference() (trainer.h:401-403, 497-502)
-	DeviceBuffer<float> ema_tmp;
-	const __half* inference_params() const { return ema.enabled ? ema_fp16.ptr : params_fp16; }
+	std::unique_ptr<Optimizer> opt;  // a module handle's is never allocated
 	float loss_scale = 128.0f;  // default_loss_scale<__half>() (common.h:243)
 	int n_sms = 132;
 
@@ -137,24 +123,10 @@ struct Model {
 	// trainer.h:489-503: one allocation [fp32 master | fp16 params | fp16 gradients]
 	DeviceBuffer<char> params_buffer;
 	size_t n_params_padded = 0;
-	bool module_only = false;  // tcnnb_module: no trainer-owned parameters / optimizer state
+	bool module_only = false;  // tcnnb_module: no trainer-owned parameters
 	float* params_fp32 = nullptr;
 	__half* params_fp16 = nullptr;
 	__half* grads_fp16 = nullptr;
-	DeviceBuffer<float> first_moments, second_moments;
-	// Per-parameter Adam step counters: 16-bit (saturating at 65535) when adam_u16_steps_exact() proves the updates identical, else
-	// 32-bit. With 16-bit counters, param_steps is the uint32 view that tcnnb_optimizer_state hands out, widened on demand; while it is
-	// live it is authoritative and is narrowed back before the next consumer (steps32 / sync_steps).
-	bool steps16 = false;
-	bool steps_mirror_live = false;
-	DeviceBuffer<uint16_t> param_steps16;
-	DeviceBuffer<uint32_t> param_steps;
-	// Calls f with the live counters (uint16_t* or uint32_t*): the Adam kernels are instantiated for both widths.
-	template <typename F>
-	void with_step_counters(F&& f) {
-		if (steps16) f(param_steps16.ptr);
-		else f(param_steps.ptr);
-	}
 	DeviceBuffer<float> dw_accum;   // fp32 MLP weight-gradient accumulator
 	DeviceBuffer<float> scalars;    // [0] = loss sum
 	DeviceBuffer<long long> dbg_clock;  // TCNNB_CLOCKS=<file> in ablation builds: phase stamps of the last ws launch
@@ -270,49 +242,6 @@ static const char* fused_kernel_unsupported(const EncodingPlan& plan, const MlpC
 	return nullptr;
 }
 
-// The uint32 step counters: the state itself, or (16-bit counters) the mirror, widened on `stream` unless it is already live.
-static uint32_t* steps32(Model& m, cudaStream_t stream) {
-	if (m.steps16 && !m.steps_mirror_live) {
-		m.param_steps.resize(m.n_params);
-		TCNNB_CUDA_CHECK(launch_widen_steps(stream, m.n_params, m.param_steps16.ptr, m.param_steps.ptr));
-		m.steps_mirror_live = true;
-	}
-	return m.param_steps.ptr;
-}
-
-// Makes the 16-bit counters current again after a caller wrote through the uint32 mirror (saturating: exact, see
-// adam_u16_steps_exact).
-static void sync_steps(Model& m, cudaStream_t stream) {
-	if (m.steps16 && m.steps_mirror_live) {
-		TCNNB_CUDA_CHECK(launch_narrow_steps(stream, m.n_params, m.param_steps.ptr, m.param_steps16.ptr));
-		m.steps_mirror_live = false;
-	}
-}
-
-// Selects the counter layout, carrying the current counts over. Synchronous.
-static void set_step_counter_width(Model& m, bool use16) {
-	if (use16 == m.steps16 && (use16 ? m.param_steps16.n : m.param_steps.n) == m.n_params) return;
-	TCNNB_CUDA_CHECK(cudaDeviceSynchronize());
-	if (use16) {
-		const bool carry = m.param_steps.n == m.n_params;
-		m.param_steps16.resize(m.n_params);
-		if (carry) TCNNB_CUDA_CHECK(launch_narrow_steps(nullptr, m.n_params, m.param_steps.ptr, m.param_steps16.ptr));
-		else m.param_steps16.zero();
-		m.param_steps.release();
-	} else {
-		m.param_steps.resize(m.n_params);
-		if (m.param_steps16.n == m.n_params) {
-			if (!m.steps_mirror_live) TCNNB_CUDA_CHECK(launch_widen_steps(nullptr, m.n_params, m.param_steps16.ptr, m.param_steps.ptr));
-		} else {
-			m.param_steps.zero();
-		}
-		m.param_steps16.release();
-	}
-	m.steps16 = use16;
-	m.steps_mirror_live = false;
-	TCNNB_CUDA_CHECK(cudaDeviceSynchronize());
-}
-
 static void build_model(Model& m, uint32_t n_in, uint32_t n_out, const json::Value& cfg, uint32_t seed, bool module_only = false) {
 	m.n_sms = require_sm90();
 #ifdef TCNNB_ENABLE_ABLATION  // profiling builds only (make ABLATION=1); the production library reads no environment switches
@@ -342,51 +271,7 @@ static void build_model(Model& m, uint32_t n_in, uint32_t n_out, const json::Val
 	else throw std::runtime_error("Loss '" + m.loss_name + "' not found");
 
 	// ---- optimizer (src/optimizer.cu:50-80, adam.h:221-303)
-	const json::Value* opt_ptr = &cfg.sub("optimizer");
-	std::string opt_name = opt_ptr->value("otype", "Adam");
-	// wrappers around the nested optimizer, in any order: ExponentialDecay (a learning-rate schedule) and Ema (averaged inference weights)
-	while (ieq(opt_name, "ExponentialDecay") || ieq(opt_name, "Ema")) {
-		if (ieq(opt_name, "ExponentialDecay")) {
-			// optimizers/exponential_decay.h:46-160: from step decay_start on, every decay_interval steps (until decay_end) the learning
-			// rate is multiplied by decay_base. Host-side bookkeeping only.
-			if (m.lr_decay.enabled) throw std::runtime_error("tcnn_b200: one ExponentialDecay wrapper per optimizer");
-			m.lr_decay.enabled = true;
-			m.lr_decay.base = (float)opt_ptr->value("decay_base", 0.1);
-			m.lr_decay.interval = (uint32_t)opt_ptr->value("decay_interval", 10000.0);
-			m.lr_decay.start = (uint32_t)opt_ptr->value("decay_start", 10000.0);
-			m.lr_decay.end = (uint32_t)opt_ptr->value("decay_end", 10000000.0);
-			if (m.lr_decay.interval == 0) throw std::runtime_error("ExponentialDecay: decay_interval must be positive.");
-		} else {
-			// optimizers/ema.h:46-200: after every step of the nested optimizer, ema = (ema * decay * (1 - decay^(t-1)) + w * (1 - decay)) /
-			// (1 - decay^t) on the working-precision weights; network->inference() reads the average (Trainer::params_inference).
-			if (m.ema.enabled) throw std::runtime_error("tcnn_b200: one Ema wrapper per optimizer");
-			m.ema.enabled = true;
-			m.ema.decay = (float)opt_ptr->value("decay", 0.99);
-			m.ema.full_precision = opt_ptr->value("full_precision", false);
-		}
-		opt_ptr = &opt_ptr->sub("nested");
-		opt_name = opt_ptr->value("otype", "Adam");
-	}
-	const json::Value& opt = *opt_ptr;
-	if (!ieq(opt_name, "Adam")) {
-		throw std::runtime_error("Optimizer '" + opt_name + "' is outside the tcnn_b200 hot path (Adam, optionally inside ExponentialDecay and / or Ema, is built)");
-	}
-	AdamParams& a = m.adam;
-	a.beta1 = (float)opt.value("beta1", (double)a.beta1);
-	a.beta2 = (float)opt.value("beta2", (double)a.beta2);
-	a.epsilon = (float)opt.value("epsilon", (double)a.epsilon);
-	a.learning_rate = (float)opt.value("learning_rate", (double)a.learning_rate);
-	a.l2_reg = (float)opt.value("l2_reg", (double)a.l2_reg);
-	a.adabound = opt.value("adabound", false);
-	a.relative_decay = (float)opt.value("relative_decay", (double)a.relative_decay);
-	a.absolute_decay = (float)opt.value("absolute_decay", (double)a.absolute_decay);
-	a.clipping_magnitude = (float)opt.value("clipping_magnitude", (double)a.clipping_magnitude);
-	a.gradient_clipping_magnitude = (float)opt.value("gradient_clipping_magnitude", (double)a.gradient_clipping_magnitude);
-	a.non_matrix_learning_rate_factor = (float)opt.value("non_matrix_learning_rate_factor", (double)a.non_matrix_learning_rate_factor);
-	a.non_matrix_l2_reg = (float)opt.value("non_matrix_l2_reg", (double)a.non_matrix_l2_reg);
-	a.optimize_matrix_params = opt.value("optimize_matrix_params", true);
-	a.optimize_non_matrix_params = opt.value("optimize_non_matrix_params", true);
-	a.skip_zero_grad_non_matrix_params = opt.value("skip_zero_grad_non_matrix_params", true);
+	m.opt = std::make_unique<Optimizer>(cfg.sub("optimizer"));
 
 	// ---- encoding, padded to the network's alignment (network_with_input_encoding.h:47; FullyFusedMLP / CutlassMLP REQUIRED_ALIGNMENT,
 	// src/network.cu:79-98). One grid or one Identity (encodings/identity.h:46-67: feature j = x_j * scale + offset, padding features
@@ -443,13 +328,6 @@ static void build_model(Model& m, uint32_t n_in, uint32_t n_out, const json::Val
 		m.params_fp32 = (float*)m.params_buffer.ptr;
 		m.params_fp16 = (__half*)(m.params_buffer.ptr + sizeof(float) * m.n_params_padded);
 		m.grads_fp16 = (__half*)(m.params_buffer.ptr + sizeof(float) * m.n_params_padded + sizeof(__half) * m.n_params_padded);
-		m.first_moments.resize(m.n_params);
-		m.first_moments.zero();
-		m.second_moments.resize(m.n_params);
-		m.second_moments.zero();
-		bool exact = false;
-		TCNNB_CUDA_CHECK(adam_u16_steps_exact(m.adam, &exact));
-		set_step_counter_width(m, exact);
 	}
 	m.dw_accum.resize(mlp.n_params);
 	m.dw_accum.zero();
@@ -466,14 +344,7 @@ static void build_model(Model& m, uint32_t n_in, uint32_t n_out, const json::Val
 		// fp32 -> fp16 (trainer.h:409-421)
 		TCNNB_CUDA_CHECK(launch_cast_params(nullptr, m.n_params, m.params_fp32, m.params_fp16));
 		++g_kernel_launches;
-		if (m.ema.enabled) {  // trainer.h:409-421: the inference parameters start as the initial parameters
-			m.ema_fp16.resize(m.n_params_padded);
-			TCNNB_CUDA_CHECK(cudaMemcpy(m.ema_fp16.ptr, m.params_fp16, sizeof(__half) * m.n_params_padded, cudaMemcpyDeviceToDevice));
-			if (m.ema.full_precision) {
-				m.ema_tmp.resize(m.n_params);
-				m.ema_tmp.zero();
-			}
-		}
+		m.opt->allocate(m.n_params, m.n_params_padded, m.params_fp16);
 	}
 	TCNNB_CUDA_CHECK(cudaDeviceSynchronize());
 	TCNNB_CUDA_CHECK(cudaStreamCreateWithFlags(&m.own_stream, cudaStreamNonBlocking));
@@ -505,83 +376,18 @@ static FusedStepParams make_params(const Model& m, uint32_t batch, uint32_t loss
 	return p;
 }
 
-// ExponentialDecay's learning-rate factor after `n_steps` uninterrupted steps: the schedule of next_adam_params replayed with the
-// same float multiplications, so that a trainer whose step count is restored continues bit-identically. Each decay boundary is
-// visited once; the loop stops early once a multiplication no longer changes the factor (0, 1 or a saturated value).
-static float lr_decay_factor_after(const Model& m, uint32_t n_steps) {
-	float factor = 1.0f;
-	if (!m.lr_decay.enabled || n_steps == 0) return factor;
-	const uint64_t last = std::min<uint64_t>((uint64_t)n_steps - 1, m.lr_decay.end);
-	for (uint64_t step = m.lr_decay.start; step <= last; step += m.lr_decay.interval) {
-		const float next = factor * m.lr_decay.base;
-		if (next == factor) break;
-		factor = next;
-	}
-	return factor;
+// What the optimizer updates: the trainer's parameter and gradient buffers, the network's gradients from the fp32 sums while they are
+// current.
+static OptimizerArrays optimizer_arrays(const Model& m) {
+	return {m.params_fp32, m.params_fp16, m.grads_fp16, m.mlp_grads_in_accum ? m.dw_accum.ptr : nullptr, m.mlp.n_params, m.loss_scale};
 }
 
-// Sets the optimizer's step count from outside (a snapshot, tcnnb_set_optimizer_progress); the decay factor follows it.
-static void restore_adam_step_count(Model& m, uint32_t n_steps) {
-	m.adam_step_count = n_steps;
-	m.lr_decay.factor = lr_decay_factor_after(m, n_steps);
-}
-
-// Hyper-parameters of the next optimizer step (advances the step counter; AdaBound bounds per adam.h:161-168).
-static AdamParams next_adam_params(Model& m) {
-	if (m.lr_decay.enabled) {  // exponential_decay.h:60-70, evaluated with the step count BEFORE this step
-		const uint32_t step = m.adam_step_count;
-		if (step == 0) m.lr_decay.factor = 1.0f;
-		if (step >= m.lr_decay.start && (step - m.lr_decay.start) % m.lr_decay.interval == 0 && step <= m.lr_decay.end) m.lr_decay.factor *= m.lr_decay.base;
-	}
-	++m.adam_step_count;
-	AdamParams a = m.adam;
-	a.learning_rate = m.adam.learning_rate * m.lr_decay.factor;
-	a.lower_lr_bound = 0;
-	a.upper_lr_bound = std::numeric_limits<float>::max();
-	if (a.adabound) {
-		a.lower_lr_bound = 0.1f - 0.1f / ((1 - a.beta2) * (float)m.adam_step_count + 1);
-		a.upper_lr_bound = 0.1f + 0.1f / ((1 - a.beta2) * (float)m.adam_step_count);
-	}
-	return a;
-}
-
-// Adam over the parameter ranges [begin, begin + count) (all parameters when n_ranges == 0). One optimizer step whatever the
-// number of ranges: the data-parallel trainer updates the MLP weights everywhere and the grid entries of its own shard only.
+// The optimizer over the parameter ranges [begin, begin + count) (all parameters when n_ranges == 0). A step that covers the network
+// weights consumes their fp32 sums.
 static void optimizer_step(Model& m, cudaStream_t stream, uint32_t n_ranges = 0, const uint64_t* begins = nullptr, const uint64_t* counts = nullptr) {
-	if (m.module_only) throw std::runtime_error("this handle was created with tcnnb_module_create: it has no optimizer.");
+	if (!m.opt->allocated()) throw std::runtime_error("this handle was created with tcnnb_module_create: it has no optimizer.");
 	m.wait_pending(stream);
-	sync_steps(m, stream);
-	const AdamParams a = next_adam_params(m);
-	const uint64_t whole_begin = 0, whole_count = m.n_params;
-	if (n_ranges == 0) {
-		n_ranges = 1;
-		begins = &whole_begin;
-		counts = &whole_count;
-	}
-	bool covers_mlp = false;
-	for (uint32_t r = 0; r < n_ranges; ++r) {
-		const uint64_t b = begins[r], c = counts[r];
-		if (b + c > m.n_params) throw std::runtime_error("optimizer_step: parameter range out of bounds.");
-		if (c == 0) continue;
-		if (b < m.mlp.n_params && b + c < m.mlp.n_params) throw std::runtime_error("optimizer_step: a range may not split the network weights.");
-		const uint32_t n_matrix = b < m.mlp.n_params ? (uint32_t)(m.mlp.n_params - b) : 0u;  // matrix weights inside this range
-		covers_mlp |= b == 0 && n_matrix > 0;
-		if (n_matrix > 0 && b != 0) throw std::runtime_error("optimizer_step: the network weights must be covered from parameter 0.");
-		float* const dw = (m.mlp_grads_in_accum && n_matrix > 0) ? m.dw_accum.ptr : nullptr;
-		m.with_step_counters([&](auto* steps) {
-			TCNNB_CUDA_CHECK(launch_adam_step(stream, a, (uint32_t)c, n_matrix, m.loss_scale, m.params_fp32 + b, m.params_fp16 + b, m.grads_fp16 + b, dw, m.first_moments.ptr + b,
-			                                  m.second_moments.ptr + b, steps + b));
-		});
-		++g_kernel_launches;
-	}
-	if (covers_mlp) m.mlp_grads_in_accum = false;
-	if (m.ema.enabled) {
-		if (n_ranges != 1 || begins[0] != 0 || counts[0] != m.n_params) throw std::runtime_error("tcnn_b200: the Ema wrapper is built for whole-vector optimizer steps (not for the sharded data-parallel optimizer)");
-		const float t = (float)m.adam_step_count;
-		TCNNB_CUDA_CHECK(launch_ema_step(stream, (uint32_t)m.n_params, m.ema.decay, 1.0f - std::pow(m.ema.decay, t - 1.0f), 1.0f / (1.0f - std::pow(m.ema.decay, t)), m.params_fp16, m.ema_fp16.ptr,
-		                                 m.ema.full_precision ? m.ema_tmp.ptr : nullptr));
-		++g_kernel_launches;
-	}
+	if (m.opt->step(stream, optimizer_arrays(m), n_ranges, begins, counts)) m.mlp_grads_in_accum = false;
 }
 
 // ---- general path: encoding kernel -> stand-alone network kernel (mlp_fused.cu), activations optionally kept for the backward pass
@@ -825,21 +631,16 @@ static void dp_training_step(Model& m, cudaStream_t stream, uint32_t shard_batch
 		// weights into every replica (multimem.st / peer stores) -> [barrier: all slices have landed everywhere; the gradient
 		// vectors may be zeroed again]. No NCCL call on the step.
 		TCNNB_CUDA_CHECK(launch_dp_barrier(stream, d.peers, ++d.epoch));
-		sync_steps(m, stream);
-		const AdamParams a = next_adam_params(m);
-		m.with_step_counters([&](auto* steps) {
-			TCNNB_CUDA_CHECK(launch_adam_step_dp(stream, a, d.peers, lo, chunk, (uint32_t)m.mlp.n_params, m.n_params, m.loss_scale, m.params_fp32, m.first_moments.ptr,
-			                                     m.second_moments.ptr, steps));
-		});
+		m.opt->step_peers(stream, d.peers, lo, chunk, optimizer_arrays(m));
 		TCNNB_CUDA_CHECK(launch_dp_barrier(stream, d.peers, ++d.epoch));
-		g_kernel_launches += 3;
+		g_kernel_launches += 2;
 		d.masters_synced = false;
 		return;
 	}
 	TCNNB_NCCL_CHECK(n.ReduceScatter(m.grads_fp16, m.grads_fp16 + lo, chunk, ncclHalf, ncclSum, d.comm_grads, stream));
 	const uint64_t begin = lo, count = lo < m.n_params ? std::min<uint64_t>(chunk, m.n_params - lo) : 0;
 	if (count) optimizer_step(m, stream, 1, &begin, &count);
-	else (void)next_adam_params(m);  // a rank with no parameters in its slice still advances the step count and the decay schedule
+	else m.opt->skip_step();  // a rank with no parameters in its slice still advances the step count and the decay schedule
 	TCNNB_CUDA_CHECK(cudaEventRecord(d.ev_updated, stream));
 	TCNNB_CUDA_CHECK(cudaStreamWaitEvent(d.gather_stream, d.ev_updated, 0));
 	TCNNB_NCCL_CHECK(n.AllGather(m.params_fp16 + lo, m.params_fp16, chunk, ncclHalf, d.comm_params, d.gather_stream));
@@ -847,6 +648,9 @@ static void dp_training_step(Model& m, cudaStream_t stream, uint32_t shard_batch
 	m.pending_params_event = d.ev_gathered;
 	d.masters_synced = false;
 }
+
+// Whether each rank holds the optimizer state of its own slice only (ZeRO-1).
+static bool optimizer_state_sharded(const Model& m) { return m.dp && m.dp->world > 1 && m.dp->shard_optimizer; }
 
 // Sum of the ranks' partial losses (each normalised over the global batch) -> the global loss, in place on every rank.
 static void dp_reduce_loss(Model& m, cudaStream_t stream) {
@@ -919,7 +723,7 @@ static void training_step_ex(Model& m, cudaStream_t stream, uint32_t batch, cons
 	c.x = x;
 	c.y = y;
 	c.data_pdf = ext_dL_dy ? nullptr : data_pdf;  // the loss is not evaluated (trainer.h:127-131)
-	c.params = use_inference_params ? m.inference_params() : m.params_fp16;
+	c.params = use_inference_params ? m.opt->inference_params(m.params_fp16) : m.params_fp16;
 	c.dL_doutput = ext_dL_dy;
 	c.mode = (GradientMode)mode;
 	c.grads = m.grads_fp16;
@@ -942,7 +746,7 @@ static void trainer_forward(Model& m, cudaStream_t stream, uint32_t batch, const
 	if (!output || (uintptr_t)output % 16 != 0) throw std::runtime_error("forward: output must be a 16-byte aligned device array.");
 	if ((uintptr_t)dL_doutput % 16 != 0) throw std::runtime_error("forward: dL_doutput must be 16-byte aligned.");
 	check_batch(batch);
-	forward(m, stream, batch, x, use_inference_params ? m.inference_params() : m.params_fp16, output, nullptr);
+	forward(m, stream, batch, x, use_inference_params ? m.opt->inference_params(m.params_fp16) : m.params_fp16, output, nullptr);
 	if (external_dL_dy || (!loss_values && !dL_doutput)) return;
 	const uint32_t pad = m.mlp.padded_out_width;
 	TCNNB_CUDA_CHECK(launch_loss(stream, m.loss_type, ACT_NONE, batch, m.n_out, pad, m.loss_scale, batch * m.n_out, output, y, data_pdf, dL_doutput, loss_values, pad, nullptr));
@@ -1062,13 +866,7 @@ static std::string make_hyperparams(const Model& m) {
 	json::Value& loss = root["loss"];
 	static const char* loss_names[] = {"L2", "RelativeL2", "L1", "RelativeL1", "Mape", "Smape", "RelativeL2Luminance", "CrossEntropy", "Variance"};
 	loss["otype"] = json::Value::string(m.loss_type < sizeof(loss_names) / sizeof(loss_names[0]) ? loss_names[m.loss_type] : m.loss_name.c_str());
-	json::Value& opt = root["optimizer"];
-	opt["otype"] = json::Value::string("Adam");
-	opt["learning_rate"] = json::Value::number(m.adam.learning_rate);
-	opt["beta1"] = json::Value::number(m.adam.beta1);
-	opt["beta2"] = json::Value::number(m.adam.beta2);
-	opt["epsilon"] = json::Value::number(m.adam.epsilon);
-	opt["l2_reg"] = json::Value::number(m.adam.l2_reg);
+	m.opt->write_hyperparams(root["optimizer"]);
 	root["n_params"] = json::Value::number((double)m.n_params);
 	root["n_mlp_params"] = json::Value::number(m.mlp.n_params);
 	root["encoded_width"] = json::Value::number(m.plan.width);
@@ -1182,13 +980,13 @@ int tcnnb_set_params_full_precision(tcnnb_model* m, const float* params, uint64_
 	TCNNB_CUDA_CHECK(cudaMemcpy(mm.params_fp32, params, sizeof(float) * n, device_ptr ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice));
 	TCNNB_CUDA_CHECK(launch_cast_params(nullptr, mm.n_params, mm.params_fp32, mm.params_fp16));
 	++g_kernel_launches;
-	if (mm.ema.enabled) TCNNB_CUDA_CHECK(cudaMemcpy(mm.ema_fp16.ptr, mm.params_fp16, sizeof(__half) * n, cudaMemcpyDeviceToDevice));  // trainer.h:415-419
+	mm.opt->reset_average(mm.params_fp16);
 	TCNNB_CUDA_CHECK(cudaDeviceSynchronize());
 	TCNNB_API_END
 }
 
 // Trainer::params_inference() (trainer.h:401-403): the Ema wrapper's averaged weights when there is one, else the working parameters.
-void* tcnnb_params_inference(tcnnb_model* m) { return (void*)m->impl.inference_params(); }
+void* tcnnb_params_inference(tcnnb_model* m) { return (void*)m->impl.opt->inference_params(m->impl.params_fp16); }
 
 int tcnnb_set_params(tcnnb_model* m, const void* params_half, uint64_t n, int device_ptr) {
 	TCNNB_API_BEGIN
@@ -1200,7 +998,7 @@ int tcnnb_set_params(tcnnb_model* m, const void* params_half, uint64_t n, int de
 	TCNNB_CUDA_CHECK(cudaMemcpy(mm.params_fp16, params_half, n * sizeof(__half), device_ptr ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice));
 	half_to_float_kernel<<<(uint32_t)((n + 255) / 256), 256>>>(n, mm.params_fp16, mm.params_fp32);
 	++g_kernel_launches;
-	if (mm.ema.enabled) TCNNB_CUDA_CHECK(cudaMemcpy(mm.ema_fp16.ptr, mm.params_fp16, sizeof(__half) * n, cudaMemcpyDeviceToDevice));  // trainer.h:428-429
+	mm.opt->reset_average(mm.params_fp16);
 	TCNNB_CUDA_CHECK(cudaDeviceSynchronize());
 	TCNNB_API_END
 }
@@ -1208,42 +1006,35 @@ int tcnnb_set_params(tcnnb_model* m, const void* params_half, uint64_t n, int de
 int tcnnb_optimizer_state(tcnnb_model* m, float** first_moments_dev, float** second_moments_dev, uint32_t** param_steps_dev, uint32_t* current_step, float* base_learning_rate) {
 	TCNNB_API_BEGIN
 	Model& mm = m->impl;
-	if (mm.module_only) throw std::runtime_error("this handle was created with tcnnb_module_create: it has no optimizer.");
-	if (mm.ema.enabled) throw std::runtime_error("tcnn_b200: snapshots of the Ema wrapper's state are not built (serialize the parameters only)");
-	if (mm.dp && mm.dp->world > 1 && mm.dp->shard_optimizer) {
-		throw std::runtime_error("optimizer state is sharded over the data-parallel ranks: each rank holds the moments of its own slice only");
-	}
+	Optimizer& opt = *mm.opt;
+	if (!opt.allocated()) throw std::runtime_error("this handle was created with tcnnb_module_create: it has no optimizer.");
+	if (opt.has_average()) throw std::runtime_error("tcnn_b200: snapshots of the Ema wrapper's state are not built (serialize the parameters only)");
+	if (optimizer_state_sharded(mm)) throw std::runtime_error("optimizer state is sharded over the data-parallel ranks: each rank holds the moments of its own slice only");
 	TCNNB_CUDA_CHECK(cudaDeviceSynchronize());
 	if (param_steps_dev) {
-		*param_steps_dev = steps32(mm, nullptr);
+		*param_steps_dev = opt.counters_u32(nullptr);
 		TCNNB_CUDA_CHECK(cudaDeviceSynchronize());
 	}
-	if (first_moments_dev) *first_moments_dev = mm.first_moments.ptr;
-	if (second_moments_dev) *second_moments_dev = mm.second_moments.ptr;
-	if (current_step) *current_step = mm.adam_step_count;
-	if (base_learning_rate) *base_learning_rate = mm.adam.learning_rate;
+	if (first_moments_dev) *first_moments_dev = opt.first_moments();
+	if (second_moments_dev) *second_moments_dev = opt.second_moments();
+	if (current_step) *current_step = opt.step_count();
+	if (base_learning_rate) *base_learning_rate = opt.base_learning_rate();
 	TCNNB_API_END
 }
 
 int tcnnb_set_optimizer_progress(tcnnb_model* m, uint32_t current_step, float base_learning_rate) {
 	TCNNB_API_BEGIN
-	if (!m->impl.module_only) {  // the caller may have just written the counters through tcnnb_optimizer_state's pointer
-		sync_steps(m->impl, nullptr);
-		TCNNB_CUDA_CHECK(cudaDeviceSynchronize());
-	}
-	restore_adam_step_count(m->impl, current_step);
-	m->impl.adam.learning_rate = base_learning_rate;
+	m->impl.opt->restore_progress(current_step, base_learning_rate);
 	TCNNB_API_END
 }
 
 // ExponentialDecay's learning-rate factor (exponential_decay.h:136-148 `learning_rate_factor`; 1 without the wrapper). Setting the
 // step count recomputes it from the schedule; a snapshot that stores its own factor restores it here afterwards.
-float tcnnb_learning_rate_factor(const tcnnb_model* m) { return m->impl.lr_decay.factor; }
+float tcnnb_learning_rate_factor(const tcnnb_model* m) { return m->impl.opt->learning_rate_factor(); }
 
 int tcnnb_set_learning_rate_factor(tcnnb_model* m, float factor) {
 	TCNNB_API_BEGIN
-	if (!m->impl.lr_decay.enabled) throw std::runtime_error("set_learning_rate_factor: the optimizer has no ExponentialDecay wrapper.");
-	m->impl.lr_decay.factor = factor;
+	m->impl.opt->set_learning_rate_factor(factor);
 	TCNNB_API_END
 }
 
@@ -1330,7 +1121,7 @@ int tcnnb_inference(tcnnb_model* m, tcnnb_stream stream, uint32_t batch_size, co
 	Model& mm = m->impl;
 	check_batch(batch_size);
 	check_trainer(mm);
-	forward(mm, (cudaStream_t)stream, batch_size, input_dev, mm.inference_params(), nullptr, output_dev);
+	forward(mm, (cudaStream_t)stream, batch_size, input_dev, mm.opt->inference_params(mm.params_fp16), nullptr, output_dev);
 	TCNNB_API_END
 }
 
@@ -1374,7 +1165,7 @@ int tcnnb_inference_host(tcnnb_model* m, uint32_t batch_size, const float* input
 	const size_t n_x = (size_t)batch_size * mm.n_in, n_y = (size_t)batch_size * mm.n_out;
 	std::memcpy(mm.pinned, input_host, n_x * sizeof(float));
 	TCNNB_CUDA_CHECK(cudaMemcpyAsync(mm.stage_in.ptr, mm.pinned, n_x * sizeof(float), cudaMemcpyHostToDevice, s));
-	forward(mm, s, batch_size, mm.stage_in.ptr, mm.inference_params(), nullptr, mm.stage_out.ptr);
+	forward(mm, s, batch_size, mm.stage_in.ptr, mm.opt->inference_params(mm.params_fp16), nullptr, mm.stage_out.ptr);
 	TCNNB_CUDA_CHECK(cudaMemcpyAsync(mm.pinned + n_x, mm.stage_out.ptr, n_y * sizeof(float), cudaMemcpyDeviceToHost, s));
 	TCNNB_CUDA_CHECK(cudaStreamSynchronize(s));
 	std::memcpy(output_host, mm.pinned + n_x, n_y * sizeof(float));
@@ -1391,15 +1182,15 @@ int tcnnb_serialize(tcnnb_model* m, void* dst_host, uint64_t size, int with_opti
 	TCNNB_API_BEGIN
 	Model& mm = m->impl;
 	if (size < tcnnb_serialize_size(m, with_optimizer)) throw std::runtime_error("tcnnb_serialize: destination too small");
-	if (with_optimizer && mm.ema.enabled) throw std::runtime_error("tcnn_b200: snapshots of the Ema wrapper's state are not built (serialize with_optimizer = 0)");
-	if (with_optimizer && mm.dp && mm.dp->world > 1 && mm.dp->shard_optimizer) {
+	if (with_optimizer && mm.opt->has_average()) throw std::runtime_error("tcnn_b200: snapshots of the Ema wrapper's state are not built (serialize with_optimizer = 0)");
+	if (with_optimizer && optimizer_state_sharded(mm)) {
 		// moments / step counters are current on the owner of a slice only (ZeRO-1): a snapshot of one rank would silently hold stale state
 		throw std::runtime_error("tcnnb_serialize: optimizer state is sharded over the data-parallel ranks; serialize with_optimizer = 0 (after tcnnb_dp_sync_full_precision) or from a single-GPU trainer");
 	}
 	TCNNB_CUDA_CHECK(cudaDeviceSynchronize());
 	char* p = (char*)dst_host;
 	const uint64_t n = mm.n_params;
-	const uint32_t wo = with_optimizer ? 1 : 0, st = mm.adam_step_count;
+	const uint32_t wo = with_optimizer ? 1 : 0, st = mm.opt->step_count();
 	std::memcpy(p, &n, 8);
 	std::memcpy(p + 8, &wo, 4);
 	std::memcpy(p + 12, &st, 4);
@@ -1407,11 +1198,11 @@ int tcnnb_serialize(tcnnb_model* m, void* dst_host, uint64_t size, int with_opti
 	TCNNB_CUDA_CHECK(cudaMemcpy(p, mm.params_fp16, n * 2, cudaMemcpyDeviceToHost));
 	p += n * 2;
 	if (with_optimizer) {
-		TCNNB_CUDA_CHECK(cudaMemcpy(p, mm.first_moments.ptr, n * 4, cudaMemcpyDeviceToHost));
+		TCNNB_CUDA_CHECK(cudaMemcpy(p, mm.opt->first_moments(), n * 4, cudaMemcpyDeviceToHost));
 		p += n * 4;
-		TCNNB_CUDA_CHECK(cudaMemcpy(p, mm.second_moments.ptr, n * 4, cudaMemcpyDeviceToHost));
+		TCNNB_CUDA_CHECK(cudaMemcpy(p, mm.opt->second_moments(), n * 4, cudaMemcpyDeviceToHost));
 		p += n * 4;
-		TCNNB_CUDA_CHECK(cudaMemcpy(p, steps32(mm, nullptr), n * 4, cudaMemcpyDeviceToHost));  // uint32 on disk whatever the counters' width
+		TCNNB_CUDA_CHECK(cudaMemcpy(p, mm.opt->counters_u32(nullptr), n * 4, cudaMemcpyDeviceToHost));  // uint32 on disk whatever the counters' width
 	}
 	TCNNB_API_END
 }
@@ -1435,15 +1226,12 @@ int tcnnb_deserialize(tcnnb_model* m, const void* src_host, uint64_t size) {
 	++g_kernel_launches;
 	p += n * 2;
 	if (wo) {
-		TCNNB_CUDA_CHECK(cudaMemcpy(mm.first_moments.ptr, p, n * 4, cudaMemcpyHostToDevice));
+		TCNNB_CUDA_CHECK(cudaMemcpy(mm.opt->first_moments(), p, n * 4, cudaMemcpyHostToDevice));
 		p += n * 4;
-		TCNNB_CUDA_CHECK(cudaMemcpy(mm.second_moments.ptr, p, n * 4, cudaMemcpyHostToDevice));
+		TCNNB_CUDA_CHECK(cudaMemcpy(mm.opt->second_moments(), p, n * 4, cudaMemcpyHostToDevice));
 		p += n * 4;
-		if (mm.steps16) mm.param_steps.resize(n);
-		TCNNB_CUDA_CHECK(cudaMemcpy(mm.param_steps.ptr, p, n * 4, cudaMemcpyHostToDevice));
-		mm.steps_mirror_live = mm.steps16;
-		sync_steps(mm, nullptr);
-		restore_adam_step_count(mm, st);
+		mm.opt->load_counters_u32((const uint32_t*)p);
+		mm.opt->restore_progress(st, mm.opt->base_learning_rate());
 	}
 	TCNNB_CUDA_CHECK(cudaDeviceSynchronize());
 	TCNNB_API_END
@@ -1462,7 +1250,7 @@ int tcnnb_dp_init(tcnnb_model* m, const void* id_grads, const void* id_params, i
 	TCNNB_API_BEGIN
 	Model& mm = m->impl;
 	if (world_size < 1 || rank < 0 || rank >= world_size) throw std::runtime_error("dp_init: bad world size / rank.");
-	if (mm.ema.enabled && world_size > 1) throw std::runtime_error("tcnn_b200: the Ema optimizer wrapper is not built for the data-parallel engines");
+	if (mm.opt->has_average() && world_size > 1) throw std::runtime_error("tcnn_b200: the Ema optimizer wrapper is not built for the data-parallel engines");
 	auto d = std::make_unique<DpState>();
 	d->world = world_size;
 	d->rank = rank;
@@ -1527,7 +1315,7 @@ int tcnnb_dp_engine(const tcnnb_model* m) {
 	return 1;
 }
 
-int tcnnb_dp_shards_optimizer(const tcnnb_model* m) { return m->impl.dp && m->impl.dp->world > 1 && m->impl.dp->shard_optimizer ? 1 : 0; }
+int tcnnb_dp_shards_optimizer(const tcnnb_model* m) { return optimizer_state_sharded(m->impl) ? 1 : 0; }
 
 int tcnnb_dp_training_step(tcnnb_model* m, tcnnb_stream stream, uint32_t shard_batch_size, uint32_t global_batch_size, const float* input_dev, const float* target_dev) {
 	TCNNB_API_BEGIN
@@ -1652,10 +1440,8 @@ int tcnnb_debug_set(tcnnb_model* m, const char* key, int value) {
 	const std::string k = key ? key : "";
 	if (k == "binning") m->impl.binning = value != 0;
 	else if (k == "adam_steps32") {  // 32-bit step counters although 16-bit ones give the same updates (tests compare the two layouts)
-		if (m->impl.module_only) throw std::runtime_error("tcnnb_debug_set(adam_steps32): this handle has no optimizer.");
-		bool exact = false;
-		if (!value) TCNNB_CUDA_CHECK(adam_u16_steps_exact(m->impl.adam, &exact));
-		set_step_counter_width(m->impl, exact);
+		if (!m->impl.opt->allocated()) throw std::runtime_error("tcnnb_debug_set(adam_steps32): this handle has no optimizer.");
+		m->impl.opt->set_counter_width(value != 0);
 	}
 	else if (k == "general") {
 		// the stand-alone kernels have their own limits (e.g. dL/d(encoded) wider than the layers): only switch when they cover the configuration
