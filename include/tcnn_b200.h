@@ -50,6 +50,16 @@ uint32_t tcnnb_abi_version(void);
  * per step, everything else on stand-alone encoding + network kernels (DESIGN.md section 3.5). Unsupported otypes fail loudly. */
 int tcnnb_create_from_config(uint32_t n_input_dims, uint32_t n_output_dims, const char* config_json, uint32_t seed, tcnnb_model** out);
 void tcnnb_destroy(tcnnb_model* model);
+/* ---- Trainer(create_network<__half>(network), optimizer, loss, seed) (trainer.h:51-87, src/network.cu:51-141): a trainer over a network
+ * alone, without an encoding. `config_json` is {"loss":{}, "optimizer":{}, "network":{}}; n_input_dims must be a multiple of 16 (the
+ * network's input width). Parameters are the network's alone and initialised like the reference's (the same pcg32 stream).
+ * Every trainer call of this header applies to the handle -- training_step(_ex), forward / backward, optimizer_step, inference,
+ * parameters, snapshots, ExponentialDecay / Ema -- with ONE difference: input_dev and dL_dinput_dev are fp16 rows
+ * [batch][n_input_dims] (the network's own input, read in place; pass them cast to float*). Targets, data_pdf and outputs are as for
+ * any handle; input and dL_dinput rows must be 16-byte aligned. The host-buffer and data-parallel calls take fp32 inputs and reject such a
+ * handle. It always runs the stand-alone
+ * network kernels. */
+int tcnnb_create_network_trainer(uint32_t n_input_dims, uint32_t n_output_dims, const char* config_json, uint32_t seed, tcnnb_model** out);
 
 /* ---- introspection (network_with_input_encoding.h:132-150, trainer.h:385-407,477-482) ---- */
 uint64_t tcnnb_n_params(const tcnnb_model* m);                 /* trainer->n_params() */
@@ -151,6 +161,12 @@ int tcnnb_optimizer_step(tcnnb_model* m, tcnnb_stream stream);
 /* generate_random_uniform<float>(stream, rng, n, out, lower, upper) (random.h:40-69) for a pcg32 with the given (state, inc):
  * thread i draws 4 consecutive numbers after advance(4 i), as the reference does. The caller advances its generator by n. */
 int tcnnb_generate_random_uniform(tcnnb_stream stream, uint64_t rng_state, uint64_t rng_inc, uint64_t n_elements, float* out_dev, float lower, float upper);
+/* generate_random_uniform<__half>: the same draws, each rounded to half and mapped as draw * (upper - lower) + lower in half arithmetic
+ * (random.h:40-69 with T = __half). out_dev is fp16 [n_elements]; lower and upper are converted to half first. */
+int tcnnb_generate_random_uniform_half(tcnnb_stream stream, uint64_t rng_state, uint64_t rng_inc, uint64_t n_elements, void* out_dev, float lower, float upper);
+/* dst [cols][rows] = src [rows][cols] transposed, for 2- or 4-byte elements (fp16 / fp32): converts between the row-major (RM) and
+ * column-major (CM) GPUMatrix layouts of the C++ object tier. src and dst must not overlap. Stream-ordered. */
+int tcnnb_transpose(tcnnb_stream stream, uint32_t rows, uint32_t cols, uint32_t element_bytes, const void* src_dev, void* dst_dev);
 
 /* ---- module tier: tcnn::cpp::Module as returned by create_network_with_input_encoding (cpp_api.h:76-125, src/cpp_api.cu:71-158) --
  * Parameters, gradients and activations are CALLER-owned device arrays (what the PyTorch extension passes, bindings.cpp:79-171):
@@ -247,6 +263,9 @@ int tcnnb_network_module_backward(tcnnb_network* n, tcnnb_stream stream, uint32_
 /* cpp::create_network semantics: fp32 input [n][n_input_dims] through the Identity encoding (padding features are 1,
  * encodings/identity.h:62-66) -> fp32 output [n][n_output_dims] (object.h:214-282). */
 int tcnnb_network_inference(tcnnb_network* n, tcnnb_stream stream, uint32_t n_elements, const float* input_dev, float* output_dev, const void* params_dev);
+/* Network<__half>::inference (object.h:214-282): fp16 input [n][n_input_dims] (a multiple of 16) -> fp32 output [n][n_output_dims], the
+ * fp16 result of tcnnb_network_inference_mixed_precision trimmed and cast. */
+int tcnnb_network_inference_half_input(tcnnb_network* n, tcnnb_stream stream, uint32_t n_elements, const void* input_dev, float* output_dev, const void* params_dev);
 /* The same with the module tier's output convention (cpp_api.cu:82-83): fp16 [n][padded_output_width]. This is what
  * tcnn::cpp::Module::inference / forward of create_network returns. */
 int tcnnb_network_module_inference(tcnnb_network* n, tcnnb_stream stream, uint32_t n_elements, const float* input_dev, void* output_dev, const void* params_dev);

@@ -28,6 +28,19 @@ public:
 	MatrixLayout layout() const { return m_layout; }
 	void memset(int value) { CUDA_CHECK_THROW(cudaMemset(m_data, value, n_bytes())); }
 	void memset_async(cudaStream_t stream, int value) { CUDA_CHECK_THROW(cudaMemsetAsync(m_data, value, n_bytes(), stream)); }
+	/* gpu_matrix.h:266-290: the elements in memory order, and a host-drawn fill (low + next_float() * (high - low), cast to T) */
+	std::vector<T> to_cpu_vector() const {
+		std::vector<T> v(n_elements());
+		CUDA_CHECK_THROW(cudaMemcpy(v.data(), m_data, n_bytes(), cudaMemcpyDeviceToHost));
+		return v;
+	}
+	template <typename RNG>
+	void initialize_uniform(RNG& rnd, float low, float high) {
+		const float scale = high - low;
+		std::vector<T> v(n_elements());
+		for (size_t i = 0; i < v.size(); ++i) v[i] = (T)(low + rnd.next_float() * scale);
+		CUDA_CHECK_THROW(cudaMemcpy(m_data, v.data(), n_bytes(), cudaMemcpyHostToDevice));
+	}
 
 protected:
 	T* m_data = nullptr;

@@ -49,11 +49,16 @@ struct pcg32 {
 
 using default_rng_t = pcg32;
 
-/* random.h:56-69: fills `out` with n uniform numbers in [lower, upper) on `stream` and advances `rng` by n */
+/* random.h:56-69: fills `out` with n uniform numbers in [lower, upper) on `stream` and advances `rng` by n. T = float or __half (each
+ * draw rounded to half, then scaled and shifted in half arithmetic, as the reference's kernel does for T = __half). */
 template <typename T, typename RNG>
 void generate_random_uniform(cudaStream_t stream, RNG& rng, size_t n_elements, T* out, const T lower = (T)0.0, const T upper = (T)1.0) {
-	static_assert(sizeof(T) == sizeof(float), "generate_random_uniform: float only");
-	TCNNB_CHECK_THROW(tcnnb_generate_random_uniform((tcnnb_stream)stream, rng.state, rng.inc, (uint64_t)n_elements, (float*)out, (float)lower, (float)upper));
+	static_assert(sizeof(T) == sizeof(float) || sizeof(T) == sizeof(__half), "generate_random_uniform: float or __half only");
+	if (sizeof(T) == sizeof(float)) {
+		TCNNB_CHECK_THROW(tcnnb_generate_random_uniform((tcnnb_stream)stream, rng.state, rng.inc, (uint64_t)n_elements, (float*)out, (float)lower, (float)upper));
+	} else {
+		TCNNB_CHECK_THROW(tcnnb_generate_random_uniform_half((tcnnb_stream)stream, rng.state, rng.inc, (uint64_t)n_elements, out, (float)lower, (float)upper));
+	}
 	rng.advance(n_elements);
 }
 

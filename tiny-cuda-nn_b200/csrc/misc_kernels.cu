@@ -59,6 +59,41 @@ __global__ void random_uniform_kernel(uint64_t n_elements, Pcg32 rng, float* __r
 	}
 }
 
+// The same for T = __half (random.h:40-69 with T = __half): the draw is rounded to half, then scaled and shifted in half arithmetic.
+__global__ void random_uniform_half_kernel(uint64_t n_elements, Pcg32 rng, __half* __restrict__ out, __half lower, __half upper) {
+	const uint64_t i = threadIdx.x + (uint64_t)blockIdx.x * blockDim.x;
+	const uint64_t n_threads = (uint64_t)blockDim.x * gridDim.x;
+	pcg_advance(rng, i * 4);
+#pragma unroll
+	for (uint64_t j = 0; j < 4; ++j) {
+		const uint64_t idx = i + n_threads * j;
+		if (idx >= n_elements) return;
+		out[idx] = __float2half(pcg_next_float(rng)) * (upper - lower) + lower;
+	}
+}
+
+// dst [cols][rows] = src [rows][cols]^T through a padded 32 x 32 shared-memory tile: both the loads and the stores are coalesced.
+// Column tiles on grid.x; row tiles on grid.y and a stride loop over it, so any number of rows fits the grid.
+template <typename T>
+__global__ void transpose_kernel(uint32_t rows, uint32_t cols, const T* __restrict__ src, T* __restrict__ dst) {
+	__shared__ T tile[32][33];
+	const uint32_t c0 = blockIdx.x * 32;
+	for (uint64_t r0 = (uint64_t)blockIdx.y * 32; r0 < rows; r0 += (uint64_t)gridDim.y * 32) {
+		for (uint32_t k = threadIdx.y; k < 32; k += blockDim.y) {
+			const uint64_t r = r0 + k;
+			const uint32_t c = c0 + threadIdx.x;
+			if (r < rows && c < cols) tile[k][threadIdx.x] = src[r * cols + c];
+		}
+		__syncthreads();
+		for (uint32_t k = threadIdx.y; k < 32; k += blockDim.y) {
+			const uint32_t c = c0 + k;
+			const uint64_t r = r0 + threadIdx.x;
+			if (r < rows && c < cols) dst[(uint64_t)c * rows + r] = tile[threadIdx.x][k];
+		}
+		__syncthreads();
+	}
+}
+
 __global__ void cast_params_kernel(uint64_t n, const float* __restrict__ in, __half* __restrict__ out) {
 	const uint64_t i = threadIdx.x + (uint64_t)blockIdx.x * blockDim.x;
 	if (i < n) out[i] = (__half)in[i];
@@ -435,6 +470,22 @@ cudaError_t launch_random_uniform(cudaStream_t stream, Pcg32 rng, uint64_t n_ele
 	if (n_elements == 0) return cudaSuccess;
 	const uint64_t n_threads = (n_elements + 3) / 4;
 	random_uniform_kernel<<<blocks_for(n_threads, 128), 128, 0, stream>>>(n_elements, rng, out, lower, upper);
+	return cudaGetLastError();
+}
+
+cudaError_t launch_random_uniform_half(cudaStream_t stream, Pcg32 rng, uint64_t n_elements, __half* out, __half lower, __half upper) {
+	if (n_elements == 0) return cudaSuccess;
+	const uint64_t n_threads = (n_elements + 3) / 4;
+	random_uniform_half_kernel<<<blocks_for(n_threads, 128), 128, 0, stream>>>(n_elements, rng, out, lower, upper);
+	return cudaGetLastError();
+}
+
+cudaError_t launch_transpose(cudaStream_t stream, uint32_t rows, uint32_t cols, uint32_t element_bytes, const void* src, void* dst) {
+	if (rows == 0 || cols == 0) return cudaSuccess;
+	const dim3 grid{(cols + 31) / 32, std::min((rows + 31) / 32, 65535u)}, block{32, 8};
+	if (element_bytes == 2) transpose_kernel<uint16_t><<<grid, block, 0, stream>>>(rows, cols, (const uint16_t*)src, (uint16_t*)dst);
+	else if (element_bytes == 4) transpose_kernel<uint32_t><<<grid, block, 0, stream>>>(rows, cols, (const uint32_t*)src, (uint32_t*)dst);
+	else return cudaErrorInvalidValue;
 	return cudaGetLastError();
 }
 

@@ -26,6 +26,10 @@ struct AdamParams {
 };
 
 cudaError_t launch_random_uniform(cudaStream_t stream, Pcg32 rng, uint64_t n_elements, float* out, float lower, float upper);
+// generate_random_uniform<__half> (random.h:40-69 with T = __half): the same stream as the float fill, rounded to half before the affine map.
+cudaError_t launch_random_uniform_half(cudaStream_t stream, Pcg32 rng, uint64_t n_elements, __half* out, __half lower, __half upper);
+// dst [cols][rows] = src [rows][cols]^T for 2- or 4-byte elements (row-major <-> column-major matrices of the C++ object tier).
+cudaError_t launch_transpose(cudaStream_t stream, uint32_t rows, uint32_t cols, uint32_t element_bytes, const void* src, void* dst);
 cudaError_t launch_cast_params(cudaStream_t stream, uint64_t n, const float* in, __half* out);
 cudaError_t launch_level_scales(cudaStream_t stream, uint32_t n_levels, float log2_per_level_scale, uint32_t base_resolution, float* scales_dev);
 // Adam's per-parameter step counters are uint32_t, or uint16_t saturating at 65535 when adam_u16_steps_exact() says that this gives

@@ -124,6 +124,9 @@ struct Model {
 	DeviceBuffer<char> params_buffer;
 	size_t n_params_padded = 0;
 	bool module_only = false;  // tcnnb_module: no trainer-owned parameters
+	// tcnnb_create_network_trainer: a Network without an encoding. The inputs (and dL/d(input)) are the network's own fp16 rows
+	// [batch][n_in], read and written in place by the stand-alone network kernels (general path).
+	bool half_input = false;
 	float* params_fp32 = nullptr;
 	__half* params_fp16 = nullptr;
 	__half* grads_fp16 = nullptr;
@@ -242,7 +245,7 @@ static const char* fused_kernel_unsupported(const EncodingPlan& plan, const MlpC
 	return nullptr;
 }
 
-static void build_model(Model& m, uint32_t n_in, uint32_t n_out, const json::Value& cfg, uint32_t seed, bool module_only = false) {
+static void build_model(Model& m, uint32_t n_in, uint32_t n_out, const json::Value& cfg, uint32_t seed, bool module_only = false, bool half_input = false) {
 	m.n_sms = require_sm90();
 #ifdef TCNNB_ENABLE_ABLATION  // profiling builds only (make ABLATION=1); the production library reads no environment switches
 	if (const char* e = std::getenv("TCNNB_ABLATE")) m.ablate = (uint32_t)std::atoi(e);
@@ -276,7 +279,13 @@ static void build_model(Model& m, uint32_t n_in, uint32_t n_out, const json::Val
 	// ---- encoding, padded to the network's alignment (network_with_input_encoding.h:47; FullyFusedMLP / CutlassMLP REQUIRED_ALIGNMENT,
 	// src/network.cu:79-98). One grid or one Identity (encodings/identity.h:46-67: feature j = x_j * scale + offset, padding features
 	// ONE) can run in the fused kernel; the plan runs every encoding on the general path and the module tier's dL/d(input).
-	const json::Value& enc_cfg = cfg.sub("encoding");
+	// A network trainer has no encoding: its plan is the parameter-free Identity of width n_in that is never run.
+	m.half_input = half_input;
+	if (half_input && (n_in == 0 || n_in % 16 != 0)) {
+		throw std::runtime_error("network trainer: fp16 inputs need n_input_dims to be a positive multiple of 16 (got " + std::to_string(n_in) + ").");
+	}
+	const json::Value identity = json::parse("{\"otype\": \"Identity\"}");
+	const json::Value& enc_cfg = half_input ? identity : cfg.sub("encoding");
 	m.enc_otype = enc_cfg.value("otype", "OneBlob");
 	build_encoding_plan(m.plan, n_in, enc_cfg, 16);
 
@@ -286,7 +295,7 @@ static void build_model(Model& m, uint32_t n_in, uint32_t n_out, const json::Val
 
 	// ---- which kernels run this configuration. The fused kernel covers the benchmarked family; everything else the stand-alone
 	// kernels cover takes the general path; the rest fails loudly (no fallback to anything that is not a kernel of this library).
-	if (const char* why = fused_kernel_unsupported(m.plan, mlp, n_in)) {
+	if (const char* why = half_input ? "fp16 network inputs" : fused_kernel_unsupported(m.plan, mlp, n_in)) {
 		m.general = true;
 		if (const char* why_not = general_path_unsupported(m)) throw std::runtime_error(std::string(why_not) + " (general path of tcnn_b200; the fused kernel does not cover this configuration: " + why + ")");
 	} else {
@@ -391,12 +400,24 @@ static void optimizer_step(Model& m, cudaStream_t stream, uint32_t n_ranges = 0,
 }
 
 // ---- general path: encoding kernel -> stand-alone network kernel (mlp_fused.cu), activations optionally kept for the backward pass
+// The network's input rows: the encoded batch, or a network trainer's own fp16 input.
+static const __half* network_input(const Model& m, const float* x) { return m.half_input ? (const __half*)x : m.g_enc.ptr; }
+
+// A network trainer's input and dL/d(input) rows go to the network kernels as they are: the same 16-byte alignment as the network tier.
+static void check_half_rows(const Model& m, const float* x, const float* dL_dinput) {
+	if (!m.half_input) return;
+	if (!x) throw std::runtime_error("network trainer: input is null.");
+	if (((uintptr_t)x | (uintptr_t)dL_dinput) % 16 != 0) throw std::runtime_error("network trainer: fp16 input / dL_dinput rows must be 16-byte aligned.");
+}
+
 static void general_forward(Model& m, cudaStream_t stream, uint32_t batch, const float* x, const __half* params, __half* out_fp16, float* out_fp32, bool keep_hidden) {
 	const MlpConfig& mlp = m.mlp;
-	grow(m.g_enc, (size_t)batch * mlp.in_width);
-	plan_forward(m.plan, stream, batch, x, params + mlp.n_params, m.g_enc.ptr, mlp.in_width, 1.0f);
+	if (!m.half_input) {
+		grow(m.g_enc, (size_t)batch * mlp.in_width);
+		plan_forward(m.plan, stream, batch, x, params + mlp.n_params, m.g_enc.ptr, mlp.in_width, 1.0f);
+	}
 	MlpForwardParams p = mlp_forward_params(mlp, params, batch, keep_hidden ? m.g_mlp.hidden_rows(mlp, batch) : nullptr);
-	p.input_fp16 = m.g_enc.ptr;
+	p.input_fp16 = network_input(m, x);  // (after the encoding's rows are grown: the pointer is read here)
 	p.output_fp16 = out_fp16;
 	p.output_fp32 = out_fp32;
 	run_mlp_forward(p, m.n_sms, stream);
@@ -461,6 +482,11 @@ static void general_backward(Model& m, cudaStream_t stream, const BackwardCall& 
 		++g_kernel_launches;
 		dL_doutput = dy_rows;
 	}
+	if (m.half_input) {  // no encoding: the network writes dL/d(input) straight into the caller's fp16 rows
+		run_mlp_backward(mlp, m.g_mlp, m.n_sms, stream, c.batch, c.params, network_input(m, c.x), m.g_mlp.hidden.ptr, out_rows, dL_doutput, c.dL_doutput != nullptr,
+		                 (__half*)c.dL_dinput, dw);
+		return;
+	}
 	const bool need_denc = table_grads || c.dL_dinput;
 	if (need_denc) grow(m.g_denc, (size_t)c.batch * mlp.in_width);
 	run_mlp_backward(mlp, m.g_mlp, m.n_sms, stream, c.batch, c.params, m.g_enc.ptr, m.g_mlp.hidden.ptr, out_rows, dL_doutput, c.dL_doutput != nullptr,
@@ -471,6 +497,7 @@ static void general_backward(Model& m, cudaStream_t stream, const BackwardCall& 
 
 // Runs one backward call on the fused kernel or the general path, then the optimizer when asked. Records one profile quadruple.
 static void backward_step(Model& m, cudaStream_t stream, const BackwardCall& c) {
+	check_half_rows(m, c.x, c.dL_dinput);
 	const uint32_t batch = c.batch, n_mlp = m.mlp.n_params;
 	const bool general = m.use_general();
 	const bool overwrite = c.mode == GRADIENT_OVERWRITE;
@@ -586,6 +613,11 @@ static void check_trainer(const Model& m) {
 	if (m.module_only) throw std::runtime_error("this handle was created with tcnnb_module_create: use the tcnnb_module_* calls.");
 }
 
+// The host-buffer and data-parallel entry points stage and shard fp32 inputs.
+static void check_float_input(const Model& m, const char* what) {
+	if (m.half_input) throw std::runtime_error(std::string(what) + " takes fp32 inputs; a network trainer (tcnnb_create_network_trainer) trains on device fp16 rows.");
+}
+
 // The trainer's own step: Overwrite into its gradient buffer (tcnnb_training_step / _shard, the host-buffer pipeline, the data-parallel
 // step).
 static void training_step(Model& m, cudaStream_t stream, uint32_t batch, uint32_t loss_batch, const float* x, const float* y, bool run_optimizer, cudaEvent_t targets_ready = nullptr) {
@@ -664,6 +696,7 @@ static void dp_reduce_loss(Model& m, cudaStream_t stream) {
 // it recomputes the forward inside the fused kernel (the gather + three MMAs per tile are cheaper than writing and re-reading
 // 2 x 64 x n fp16 activations, which is what the reference's context holds).
 static void forward(Model& m, cudaStream_t stream, uint32_t batch, const float* x, const __half* params, __half* out_fp16, float* out_fp32) {
+	check_half_rows(m, x, nullptr);
 	m.wait_pending(stream);
 	if (m.use_general()) {
 		general_forward(m, stream, batch, x, params, out_fp16, out_fp32, false);
@@ -779,6 +812,7 @@ static bool host_ptr_is_pinned(Model& m, const void* ptr) {
 // landed, the fused kernel when the targets have), the loss read-back behind it. At most two steps are in flight.
 static uint64_t host_step_submit(Model& m, uint32_t batch, uint32_t global_batch, const float* x_host, const float* y_host, bool data_parallel) {
 	check_batch(batch);
+	check_float_input(m, "the host-buffer training step");
 	const uint64_t ticket = m.next_ticket;
 	Model::HostSlot& sl = m.slots[ticket & 1u];
 	if (sl.busy) throw std::runtime_error("training_step_host_submit: two steps are already in flight; collect ticket " + std::to_string(sl.ticket) + " with tcnnb_training_step_host_wait first.");
@@ -911,6 +945,17 @@ int tcnnb_create_from_config(uint32_t n_input_dims, uint32_t n_output_dims, cons
 	const json::Value cfg = json::parse(config_json ? config_json : "{}");
 	std::unique_ptr<tcnnb_model> m{new tcnnb_model{}};
 	build_model(m->impl, n_input_dims, n_output_dims, cfg, seed);
+	*out = m.release();
+	TCNNB_API_END
+}
+
+int tcnnb_create_network_trainer(uint32_t n_input_dims, uint32_t n_output_dims, const char* config_json, uint32_t seed, tcnnb_model** out) {
+	TCNNB_API_BEGIN
+	if (!out) throw std::runtime_error("tcnnb_create_network_trainer: out is null");
+	*out = nullptr;
+	const json::Value cfg = json::parse(config_json ? config_json : "{}");
+	std::unique_ptr<tcnnb_model> m{new tcnnb_model{}};
+	build_model(m->impl, n_input_dims, n_output_dims, cfg, seed, /*module_only=*/false, /*half_input=*/true);
 	*out = m.release();
 	TCNNB_API_END
 }
@@ -1160,6 +1205,7 @@ int tcnnb_inference_host(tcnnb_model* m, uint32_t batch_size, const float* input
 	Model& mm = m->impl;
 	check_batch(batch_size);
 	check_trainer(mm);
+	check_float_input(mm, "tcnnb_inference_host");
 	ensure_staging(mm, batch_size);
 	cudaStream_t s = mm.own_stream;
 	const size_t n_x = (size_t)batch_size * mm.n_in, n_y = (size_t)batch_size * mm.n_out;
@@ -1250,6 +1296,7 @@ int tcnnb_dp_init(tcnnb_model* m, const void* id_grads, const void* id_params, i
 	TCNNB_API_BEGIN
 	Model& mm = m->impl;
 	if (world_size < 1 || rank < 0 || rank >= world_size) throw std::runtime_error("dp_init: bad world size / rank.");
+	check_float_input(mm, "data-parallel training");
 	if (mm.opt->has_average() && world_size > 1) throw std::runtime_error("tcnn_b200: the Ema optimizer wrapper is not built for the data-parallel engines");
 	auto d = std::make_unique<DpState>();
 	d->world = world_size;
@@ -1350,6 +1397,28 @@ int tcnnb_generate_random_uniform(tcnnb_stream stream, uint64_t rng_state, uint6
 	rng.state = rng_state;
 	rng.inc = rng_inc;
 	TCNNB_CUDA_CHECK(launch_random_uniform((cudaStream_t)stream, rng, n_elements, out_dev, lower, upper));
+	++g_kernel_launches;
+	TCNNB_API_END
+}
+
+int tcnnb_generate_random_uniform_half(tcnnb_stream stream, uint64_t rng_state, uint64_t rng_inc, uint64_t n_elements, void* out_dev, float lower, float upper) {
+	TCNNB_API_BEGIN
+	if (n_elements && !out_dev) throw std::runtime_error("generate_random_uniform: out is null.");
+	Pcg32 rng;
+	rng.state = rng_state;
+	rng.inc = rng_inc;
+	TCNNB_CUDA_CHECK(launch_random_uniform_half((cudaStream_t)stream, rng, n_elements, (__half*)out_dev, __float2half(lower), __float2half(upper)));
+	++g_kernel_launches;
+	TCNNB_API_END
+}
+
+int tcnnb_transpose(tcnnb_stream stream, uint32_t rows, uint32_t cols, uint32_t element_bytes, const void* src_dev, void* dst_dev) {
+	TCNNB_API_BEGIN
+	if (element_bytes != 2 && element_bytes != 4) throw std::runtime_error("transpose: element_bytes must be 2 or 4.");
+	if (rows == 0 || cols == 0) return 0;
+	if (!src_dev || !dst_dev) throw std::runtime_error("transpose: src / dst is null.");
+	if (src_dev == dst_dev) throw std::runtime_error("transpose: src and dst must not be the same array.");
+	TCNNB_CUDA_CHECK(launch_transpose((cudaStream_t)stream, rows, cols, element_bytes, src_dev, dst_dev));
 	++g_kernel_launches;
 	TCNNB_API_END
 }

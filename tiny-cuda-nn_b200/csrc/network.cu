@@ -292,6 +292,19 @@ int tcnnb_network_module_inference(tcnnb_network* n, tcnnb_stream stream, uint32
 	TCNNB_API_END
 }
 
+int tcnnb_network_inference_half_input(tcnnb_network* n, tcnnb_stream stream, uint32_t n_elements, const void* input_dev, float* output_dev, const void* params_dev) {
+	TCNNB_API_BEGIN
+	const Network& net = n->impl;
+	if (net.n_input_dims != net.cfg.in_width) throw std::runtime_error("network: fp16 inputs need n_input_dims to be a multiple of 16.");
+	if (!input_dev || !output_dev) throw std::runtime_error("network: input / output is null.");
+	if ((uintptr_t)input_dev % 16 != 0) throw std::runtime_error("network: input must be 16-byte aligned.");
+	MlpForwardParams p = make_params(net, n_elements, params_dev);
+	p.input_fp16 = (const __half*)input_dev;
+	p.output_fp32 = output_dev;
+	run_mlp_forward(p, net.n_sms, (cudaStream_t)stream);
+	TCNNB_API_END
+}
+
 int tcnnb_network_inference(tcnnb_network* n, tcnnb_stream stream, uint32_t n_elements, const float* input_dev, float* output_dev, const void* params_dev) {
 	TCNNB_API_BEGIN
 	const Network& net = n->impl;

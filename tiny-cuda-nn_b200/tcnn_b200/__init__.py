@@ -44,6 +44,7 @@ ABI = [
     ("tcnnb_set_cuda_device", _int, [_int]),
     ("tcnnb_abi_version", _u32, []),
     ("tcnnb_create_from_config", _int, [_u32, _u32, ctypes.c_char_p, _u32, ctypes.POINTER(_vp)]),
+    ("tcnnb_create_network_trainer", _int, [_u32, _u32, ctypes.c_char_p, _u32, ctypes.POINTER(_vp)]),
     ("tcnnb_destroy", None, [_vp]),
     ("tcnnb_n_params_padded", ctypes.c_uint64, [_vp]),
     ("tcnnb_n_params", _u64, [_vp]),
@@ -72,6 +73,8 @@ ABI = [
     ("tcnnb_training_step_shard", _int, [_vp, _vp, _u32, _u32, _vp, _vp, _int]),
     ("tcnnb_optimizer_step", _int, [_vp, _vp]),
     ("tcnnb_generate_random_uniform", _int, [_vp, ctypes.c_uint64, ctypes.c_uint64, ctypes.c_uint64, _vp, ctypes.c_float, ctypes.c_float]),
+    ("tcnnb_generate_random_uniform_half", _int, [_vp, ctypes.c_uint64, ctypes.c_uint64, ctypes.c_uint64, _vp, ctypes.c_float, ctypes.c_float]),
+    ("tcnnb_transpose", _int, [_vp, _u32, _u32, _u32, _vp, _vp]),
     ("tcnnb_module_create", _int, [ctypes.c_uint32, ctypes.c_uint32, ctypes.c_char_p, ctypes.c_char_p, ctypes.POINTER(_vp)]),
     ("tcnnb_module_initialize_params", _int, [_vp, ctypes.c_uint64, _vp, ctypes.c_float]),
     ("tcnnb_module_inference", _int, [_vp, _vp, ctypes.c_uint32, _vp, _vp, _vp]),
@@ -102,6 +105,7 @@ ABI = [
     ("tcnnb_network_backward", _int, [_vp, _vp, _u32, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     ("tcnnb_network_module_backward", _int, [_vp, _vp, _u32, _vp, _vp, _vp, _vp, _vp]),
     ("tcnnb_network_inference", _int, [_vp, _vp, _u32, _vp, _vp, _vp]),
+    ("tcnnb_network_inference_half_input", _int, [_vp, _vp, _u32, _vp, _vp, _vp]),
     ("tcnnb_network_debug_clocks", _int, [_vp, _vp]),
     ("tcnnb_network_debug_grad_hidden", _int, [_vp, _vp]),
     ("tcnnb_network_module_inference", _int, [_vp, _vp, _u32, _vp, _vp, _vp]),
